@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — LSIGF edge·feature ops/s on B200 (BASELINE.json `metric`), with roofline, parity check and CPU baseline.
+"""bench.py — LSIGF edge·feature ops/s on H100 (BASELINE.json `metric`), with roofline, parity check and CPU baseline.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload er1m|cfg2|cfg3|cfg4|er2m|sbm1m] [--impl reference]
 
@@ -12,14 +12,15 @@ A "step" is one LSIGF forward (alegnn/utils/graphML.py:83-176 semantics) over on
            timed region, overlapped ACROSS steps on two copy streams (class E2EPipeline).
   roofline = the shift kernel: algorithmic bytes per launch (gather model, SURVEY.md §8d) divided by its average
            duration measured live with CUDA events around every hop launch inside the timed region (events recorded
-           by the library on the launching stream), against MEASURED_PEAKS.json's HBM copy bandwidth.
+           by the library on the launching stream), against MEASURED_PEAKS.json's HBM copy bandwidth when present, else
+           the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s).
   parity_max_rel = max|y - y_ref| / max|y_ref| of the timed path's output against the fp64 CPU oracle
            (oracle/lsigf_oracle.py:lsigf_sparse_stream) at the FULL workload size, at every N (the ranks' rows are
            gathered); the run fails above 1e-4.  `selftest` (N > 1): forward AND backward of both shardings against the
            oracle on a small graph, over NCCL / NVLink on the same ranks.
   cpu_baseline = the reference's dense torch.matmul algorithm (oracle/lsigf_oracle.py:lsigf_dense_torch, a port: the
-           reference is Python, cannot be pip-installed offline — DESIGN.md §6 — and cannot travel to the GPU box) on this
-           box's host cores, bounded sample, thread count pinned and printed.
+           reference is Python, cannot be pip-installed offline — DESIGN.md §6 — and is not part of this repository) on
+           the GPU machine's host cores, bounded sample, thread count pinned and printed.
   configs = at N = 1 the other single-GPU configurations of BASELINE.json (cfg2, cfg3, cfg4; cfg4ev = config 4 as the
            reference's EdgeVariantGF layer) measured the same way in the same run (fewer steps), each with its own parity.
 Default workload = the configuration the north_star target is quoted on: ER N=1M, avgDeg=32, K=5, G=F=64, B=1, fp32.
@@ -51,6 +52,7 @@ WORKLOADS = {
     "sbm1m": dict(graph="sbm", N=1_000_000, deg=32, E=1, K=5, G=64, F=64, B=1, seed=6, communities=1000, intra=0.8),
 }
 PARITY_TOL = 1e-4      # north_star tolerance (fp32); fp64 runs are held to 1e-10
+L2_BYTES = 50 * 2 ** 20  # H100 SXM L2
 
 
 def describe(w, dtype="f32"):
@@ -84,7 +86,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def usable_cores():
@@ -426,7 +428,7 @@ def ctypes_floats(lib, plan, n):
 
 def load_ncu_traffic(workload, dtype):
     """DRAM bytes per hop launch (dram__bytes_read.sum + dram__bytes_write.sum) from the committed `ncu --set full`
-    capture of this workload / dtype / kernel version (profiles/ncu_traffic.json names the capture file), or null."""
+    capture of this workload / dtype / kernel version (profiles/ncu_traffic.json, when one is on file), or null."""
     p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     try:
         d = json.load(open(p))
@@ -461,8 +463,9 @@ def hop_roofline(ctx, hop_ms, step_ms_total, nnz, rows, C, kernel, workload=None
     return out
 
 
-def single_gpu_workload(ctx, name, w, steps, warmup, full):
-    """One workload on one GPU: timed forward (+ hop profile, parity; with `full` also e2e and forward+backward)."""
+def single_gpu_workload(ctx, name, w, steps, warmup, full, keep_last=False):
+    """One workload on one GPU: timed forward (+ hop profile, parity; with `full` also e2e and forward+backward).
+    keep_last: the output of the last timed step is returned as res["last_output"]."""
     import gnn_b200
     args, dev, tdt, es, lib = ctx.args, ctx.dev, ctx.tdt, ctx.es, ctx.lib
     E, K, G, F, B, N = w["E"], w["K"], w["G"], w["F"], w["B"], w["N"]
@@ -476,17 +479,24 @@ def single_gpu_workload(ctx, name, w, steps, warmup, full):
     x = x_cpu.to(dev)                                         # reference layout, resident in HBM
     plan = gso.plan(dev)
     fwd = lambda: gnn_b200.LSIGF(h, gso, x, b)               # noqa: E731  (layout conversion inside the step)
+    last = []
+
+    def fwd_keep():
+        last[:] = [fwd()]
+
     hops = E * (K - 1)
     cap = hops * (steps + warmup)
     lib.b200gf_profile_hops(plan.handle, cap)
     with torch.no_grad(), ClockSampler(ctx.local) as clk:
-        ms, launches = ctx.timed(fwd, steps, warmup)
+        ms, launches = ctx.timed(fwd_keep if keep_last else fwd, steps, warmup)
     hop_ms = ctypes_floats(lib, plan, cap)[hops * warmup:]   # launches inside the timed region only
     lib.b200gf_profile_hops(plan.handle, 0)
     rf = hop_roofline(ctx, hop_ms, ms * steps, nnz_e, N, B * G, "spmm_hop_v2_kernel" if B * G * es > 128
                       else "spmm_hop_multirow_kernel", workload=name)
     out = {"ms_per_step": ms, "value": ops_per_step / (ms * 1e-3), "unit": "edge-feature-op/s", "nnz": gso.nnz(),
            "ops_per_step": ops_per_step, "gpu_launches": launches, "clocks": clk.summary(), "roofline": rf}
+    if keep_last:
+        out["last_output"] = last[0]
     if not args.no_check:
         t0 = time.time()
         with torch.no_grad():
@@ -522,7 +532,7 @@ def single_gpu_workload(ctx, name, w, steps, warmup, full):
                           "value": float(gso.nnz()) * (K - 1) * B * (G + F) / (ms_fb * 1e-3),
                           "note": "forward hops on B*G columns + backward hops on B*F columns per step"}
     out["l2"] = ("inputs larger than L2 (x and every z_k are %d MB each; no flush needed)" % (N * B * G * es // 2 ** 20)
-                 if N * B * G * es > 126 * 2 ** 20 else "working set fits L2: numbers are L2-warm")
+                 if N * B * G * es > L2_BYTES else "working set fits L2: numbers are L2-warm")
     return out, gso
 
 
@@ -864,7 +874,7 @@ def multi_gpu_arm(ctx, w, out_fd):
             "scaling": "strong", "vs_baseline": None, "dtype": args.dtype, "data": "synthetic",
             "config": {"workload": describe(w, args.dtype), "name": args.workload, "nnz": gso.nnz(), "parallelism": parallelism,
                        "l2": "inputs larger than L2 (x and every z_k are %d MB each; no flush needed)" % (N * B * G * es // 2 ** 20)
-                       if N * B * G * es > 126 * 2 ** 20 else "working set fits L2: numbers are L2-warm",
+                       if N * B * G * es > L2_BYTES else "working set fits L2: numbers are L2-warm",
                        "ops_per_step": ops_per_step,
                        "note": "x is the node-major shard each rank owns (layout conversion is not part of the N > 1 step)"},
             "gpu_launches": int(lt.item()),
@@ -891,12 +901,33 @@ def multi_gpu_arm(ctx, w, out_fd):
         sys.exit(code)
 
 
+DUMP_BYTES = 32 * 2 ** 20   # what --dump-outputs writes at most (all files together stay far below 64 MB)
+
+
+def dump_outputs(dirname, y):
+    """Writes the timed path's output y [B, F, N] (what LSIGF returns) to DIR/y.npy in its own float type: all of it when it
+    fits DUMP_BYTES, else the columns of a fixed seeded sample of nodes, sorted, whose indices go to DIR/y_nodes.npy
+    (float64, exact).  Inputs are seeded, so two builds run with the same arguments can be compared file by file."""
+    os.makedirs(dirname, exist_ok=True)
+    B, F, N = y.shape
+    es = y.element_size()
+    n = min(N, max(1, DUMP_BYTES // (B * F * es)))
+    if n < N:
+        nodes = np.sort(np.random.default_rng(0).choice(N, n, replace=False))
+        y = y[:, :, torch.from_numpy(nodes).to(y.device)]
+        np.save(os.path.join(dirname, "y_nodes.npy"), nodes.astype(np.float64))
+    np.save(os.path.join(dirname, "y.npy"), y.detach().cpu().numpy())
+
+
 def run_gpu_arm(args, w):
     out_fd = _JsonOnlyStdout()
     ctx = Ctx(args)
     if ctx.world > 1:
         return multi_gpu_arm(ctx, w, out_fd)
-    res, gso = single_gpu_workload(ctx, args.workload, w, args.steps, args.warmup, full=True)
+    res, gso = single_gpu_workload(ctx, args.workload, w, args.steps, args.warmup, full=True,
+                                   keep_last=bool(args.dump_outputs))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, res.pop("last_output"))
     line = {
         "metric": "LSIGF edge-feature ops/s", "value": res["value"], "unit": "edge-feature-op/s",
         "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": res["ms_per_step"], "higher_is_better": True,
@@ -965,6 +996,9 @@ def main():
     ap.add_argument("--dtype", default="f32", choices=["f32", "f64"], help="arithmetic type (headline: f32)")
     ap.add_argument("--configs", default="cfg2,cfg3,cfg4,cfg4ev",
                     help="N = 1: other BASELINE.json configurations measured in the same run ('' = none)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's output to DIR/*.npy (single GPU; a seeded sample of "
+                         "nodes when it is larger than 32 MB)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-full-size-cpu", action="store_true", help="reference arm: skip the full-size sparse CPU figure")
     ap.add_argument("--no-check", action="store_true", help="skip the full-size parity check against the CPU oracle")
@@ -979,6 +1013,8 @@ def main():
     ap.add_argument("--symm", default="auto", choices=["auto", "torch", "ipc"],
                     help="node sharding: symmetric memory through torch (multicast when available) or plain CUDA IPC")
     args = ap.parse_args()
+    if args.dump_outputs and (args.gpus != 1 or args.impl != "b200"):
+        ap.error("--dump-outputs is for the single-GPU CUDA path (--gpus 1)")
     args.warmup = max(3, args.warmup)
     w = WORKLOADS[args.workload]
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-"""b200gf — B200-native LSIGF graph-filter path (drop-in for alegnn.utils.graphML.LSIGF / GraphFilter).
+"""b200gf — H100-native LSIGF graph-filter path (drop-in for alegnn.utils.graphML.LSIGF / GraphFilter).
 
 The directory is called `graph-neural-networks_b200` (not a valid Python identifier); import it through the
 `gnn_b200` loader module at the repo root:  `import gnn_b200 as b200`.

@@ -1,4 +1,4 @@
-"""ctypes binding of include/b200gf.h (libb200gf.so, built by build.py with nvcc for sm_100a).
+"""ctypes binding of include/b200gf.h (libb200gf.so, built by build.py with nvcc for sm_90a).
 
 There is NO fallback: if the library is missing `load()` raises, and every LSIGF call raises with it.
 """

@@ -1,4 +1,4 @@
-// Internal helpers shared by the b200gf translation units (sm_100a only).
+// Internal helpers shared by the b200gf translation units (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -93,7 +93,7 @@ int launch_bias_grad(int dtype, int64_t n_rows, int B, int F, const void* dy, in
                      int bias_per_node, void* scratch, size_t scratch_bytes, cudaStream_t st);
 size_t bias_grad_scratch_bytes(int dtype, int64_t n_rows, int B, int F);
 
-// tensor-core (tcgen05, 3xTF32) contraction, tc_contract.cu
+// tensor-core (wgmma, 3xTF32) contraction, tc_contract.cu
 size_t tc_contract_scratch_bytes(int T, int P, int Q);
 bool tc_contract_eligible(int dtype, int64_t n_rows, int B, int P, int Q, int T, const void* const* zs,
                           const int64_t* z_ld, const void* out, int64_t out_ld, int accumulate);
@@ -124,7 +124,7 @@ struct b200gf_plan {
   int dtype = B200GF_F32;
   int64_t n_rows = 0, n_cols = 0;
   int E = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   bool symmetric = false;
   bool has_bwd = false;
   std::vector<b200gf::CsrDev> fwd;  // CSR of S_e^T rows: forward shift gather operator

@@ -3,9 +3,7 @@
 //
 //     out[(n,b), q] = act( bias + sum_t sum_p Z_t[(n,b), p] * W[t][p][q] )       (graphML.py:170-175)
 //
-// replaces tap_contract_kernel<double> (4x4 register-tile FMA, 4.2 ms at N = 1M, T = 5, P = Q = 64) when eligible:
-// 1.42 ms in the standalone probe this kernel grew out of (profiles/r2_probe_contract_f64.log; bounds: 41 GFLOP at the
-// FP64 peak ~ 1 ms, 3.1 GB of operands ~ 0.5 ms).
+// replaces tap_contract_kernel<double> (4x4 register-tile FMA) when eligible.
 //
 // Mapping: persistent CTAs (256 threads, one per SM and 64-column block of Q).  The taps of the CTA's column block,
 // W[T][P][64], stay in shared memory for the whole kernel (row pitch 68 doubles: the four k-rows of a B fragment land 8

@@ -78,8 +78,7 @@ step_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ col,
     const T* __restrict__ up = (k == 0 ? xT : uprev + (size_t)f * G * plane) + b;      // + g * plane
     T* __restrict__ uc = ucur ? ucur + (size_t)f * G * plane + (size_t)i * B + b : nullptr;
     // GB input features at a time: their loads (one weight + one state row each per non-zero) are independent, so GB
-    // requests are in flight per thread instead of one (ncu on the one-g-at-a-time loop: 88 % long-scoreboard stalls,
-    // 0.32 eligible warps per scheduler, DRAM at 26 % — profiles/r2_prof_ev_step_details.txt)
+    // requests are in flight per thread instead of one (the one-g-at-a-time loop stalls on each load in turn)
     for (int g0 = 0; g0 < G; g0 += GB) {
       BVec<T, VB> acc[GB];
 #pragma unroll
@@ -244,7 +243,7 @@ xgrad_kernel(const int64_t* __restrict__ rowptrT, const int32_t* __restrict__ co
   }
 }
 
-inline int grid_for(int64_t total) { return (int)imin64((total + 255) / 256, 148 * 16); }
+inline int grid_for(int64_t total) { return (int)imin64((total + 255) / 256, 132 * 16); }
 
 // 16-byte batch vectors: float data, B a multiple of 4, every operand 16-byte aligned (all row strides are multiples of B)
 template <typename T>
@@ -287,7 +286,7 @@ int backward_t(int64_t NA, int B, int G, int F, int K, const int64_t* rowptr, co
   const int64_t items = (int64_t)F * G * NA;
   for (int k = K - 1; k >= 0; --k) {
     if (nnz > 0) {
-      const int blocks = (int)imin64((items + 7) / 8, 148 * 16);
+      const int blocks = (int)imin64((items + 7) / 8, 132 * 16);
       wgrad_kernel<T><<<blocks, 256, 0, st>>>(rowptr, col, diag, cur, k > 0 ? states + (int64_t)(k - 1) * chain : nullptr, xT, dw,
                                               NA, B, G, K, k, nnz, items);
       LAUNCH_CHECK();

@@ -55,7 +55,7 @@ __global__ void maxpool_bwd_kernel(const T* __restrict__ dy, int64_t dy_ld, cons
   }
 }
 
-inline int grid_for(int64_t total) { return (int)imin64((total + 255) / 256, 148LL * 16); }
+inline int grid_for(int64_t total) { return (int)imin64((total + 255) / 256, 132LL * 16); }
 
 }  // namespace layer
 }  // namespace b200gf

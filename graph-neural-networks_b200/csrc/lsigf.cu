@@ -3,7 +3,7 @@
 // all scratch lives in the caller-provided workspace, so a call is CUDA-graph capturable.
 //
 // Forward   z_{e,0} = x ; z_{e,k} = z_{e,k-1} · S_e   (K-1 hops per edge feature, spmm.cu)
-//           y = sum_{e,k} z_{e,k} · h[:,e,k,:]^T + b   (tap contraction; tcgen05 3xTF32 when eligible, FMA otherwise)
+//           y = sum_{e,k} z_{e,k} · h[:,e,k,:]^T + b   (tap contraction; wgmma 3xTF32 when eligible, FMA otherwise)
 // Backward  V_{e,0} = dy ; V_{e,k} = V_{e,k-1} · S_e^T (K-1 hops with the other operator)
 //           dx = sum_{e,k} V_{e,k} · h[:,e,k,:]        dh[f,e,k,g] = sum_{b,n} V_{e,k}[b,f,n] x[b,g,n]
 //           db = sum dy.   Only x is needed from the forward: no z_{e,k} is saved.
@@ -190,7 +190,7 @@ static int forward_impl(const b200gf_plan* plan, const void* x, int x_layout, in
   void* yo = y_layout == B200GF_NODE_MAJOR ? y : w.yn;
   const int64_t yo_ld = y_layout == B200GF_NODE_MAJOR ? y_ld : ldf;
   if (tc_contract_eligible(dt, N, B, G, F, T, zs.data(), zld.data(), yo, yo_ld, 0)) {
-    // tensor cores: tcgen05 3xTF32, operands K-major: W[t][f][g]
+    // tensor cores: wgmma 3xTF32, operands K-major: W[t][f][g]
     if ((rc = launch_pack_taps_split(h, w.W, F, E, K, G, 0, st))) return rc;
     if ((rc = launch_tc_contract(plan->sm_count, N, B, G, F, T, zs.data(), w.W, bias, bias_per_node, yo, yo_ld, st, act)))
       return rc;

@@ -110,7 +110,7 @@ int init_device(b200gf_plan* p, int device) {
   }
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10) return B200GF_ENODEVICE;  // built for sm_100a only
+  if (prop.major != 9 || prop.minor != 0) return B200GF_ENODEVICE;  // built for sm_90a only
   CUDA_TRY(cudaSetDevice(device));
   p->device = device;
   p->sm_count = prop.multiProcessorCount;
@@ -150,7 +150,7 @@ const char* b200gf_strerror(int rc) {
     case B200GF_EUNSUPPORTED: return "b200gf: unsupported dtype or size";
     case B200GF_ENOMEM: return "b200gf: out of memory";
     case B200GF_EWORKSPACE: return "b200gf: workspace too small";
-    case B200GF_ENODEVICE: return "b200gf: no sm_100 CUDA device";
+    case B200GF_ENODEVICE: return "b200gf: no sm_90 CUDA device";
     default: break;
   }
   if (rc <= B200GF_ECUDA) {
@@ -272,7 +272,7 @@ int adopt(const int64_t* rowptr, const int32_t* col, const void* val, int64_t n_
   }
   if (nnz < (int64_t)INT32_MAX) {
     if (cudaMalloc(&D.rowptr32, (size_t)(n_rows + 1) * sizeof(int32_t)) != cudaSuccess) return B200GF_ENOMEM;
-    narrow_rowptr_kernel<<<(int)imin64((n_rows + 256) / 256, 1184), 256>>>(D.rowptr, D.rowptr32, n_rows + 1);
+    narrow_rowptr_kernel<<<(int)imin64((n_rows + 256) / 256, 132 * 8), 256>>>(D.rowptr, D.rowptr32, n_rows + 1);
     LAUNCH_CHECK();
   }
   return B200GF_OK;

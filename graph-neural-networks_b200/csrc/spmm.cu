@@ -3,7 +3,7 @@
 // and src/dst node-major [rows, ld] feature matrices.  This replaces the reference's dense broadcast-batched
 // GEMM torch.matmul(x, S) and is the HBM-bound kernel the roofline in bench.py is quoted on.
 //
-// Mapping (sm_100a, 148 SMs) — details and the measured alternatives in spmm_kernels.cuh / profiles/README.md:
+// Mapping (sm_90a, 132 SMs) — details in spmm_kernels.cuh:
 //   * rows of more than 128 bytes: one warp per (row, column chunk), chunk-major grid-stride order (keeps the gathered
 //     column slab L2-resident when it fits), L lanes x 16-byte vectors per neighbour row, 32/L neighbours per LDG.128,
 //     U loads in flight per lane, col/val read once per row and broadcast by SHFL, 48 resident warps per SM,
@@ -16,7 +16,7 @@
 #include "common.cuh"
 #include "spmm_kernels.cuh"
 
-// L2 policy of the gathered rows in the v2 kernel (spmm_kernels.cuh HINT codes), chosen from profiles/r2_spmm_sweep2_c64.log
+// L2 policy of the gathered rows in the v2 kernel (spmm_kernels.cuh HINT codes)
 #ifndef B200GF_HOP_L2_HINT
 #define B200GF_HOP_L2_HINT 3
 #endif
@@ -46,10 +46,9 @@ static BcastArgs<T> make_bcast(const BcastHost* bh) {
   return bc;
 }
 
-// Library configuration, chosen from tools/spmm_sweep.cu on B200 (profiles/r1_spmm_sweep.md): 256 threads,
-// registers capped for 6 resident blocks/SM (48 warps: the kernel is latency-bound below that), gathered rows loaded
-// with an L2 evict_last policy and no L1 allocation (DRAM reads 7.9 GB -> 6.3 GB per hop at N=1M, C=64), no
-// next-row prefetch (it costs registers and measured slower).
+// Library configuration (tools/spmm_sweep.cu explores the alternatives): 256 threads, registers capped for 6 resident
+// blocks/SM (48 warps: the kernel is latency-bound below that), gathered rows loaded with an L2 evict_last policy and no
+// L1 allocation (a sticky subset of the gathered slab stays in L2), no next-row prefetch (it costs registers).
 template <typename T, int VEC, int L, int U>
 static int launch_one(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst,
                       int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh) {
@@ -72,8 +71,8 @@ static int launch_one(int sm_count, const CsrDev& A, int64_t n_rows, const T* sr
   return B200GF_OK;
 }
 
-// narrow rows (<= 128 bytes): several rows per warp (spmm_hop_multirow_kernel); geometry from the small-C sweep
-// (profiles/r1_spmm_sweep_smallC.log: C = 8 0.39 -> 0.19 ms, C = 16 0.48 -> 0.34 ms, C = 32 0.75 -> 0.68 ms at N = 1M)
+// narrow rows (<= 128 bytes): several rows per warp (spmm_hop_multirow_kernel), geometry from the small-C sweep of
+// tools/spmm_sweep.cu
 template <typename T, int VEC, int L, int GS, int U, int MINB>
 static int launch_multirow(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst,
                            int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh) {
@@ -93,9 +92,9 @@ static int launch_multirow(int sm_count, const CsrDev& A, int64_t n_rows, const 
   return B200GF_OK;
 }
 
-// Round-2 kernel (spmm_kernels.cuh: spmm_hop_v2_kernel): 32-byte lanes (LDG.E.256), 32-bit index arithmetic, no spills.
+// Round-2 kernel (spmm_kernels.cuh: spmm_hop_v2_kernel): 32-byte lanes (two adjacent LDG.128), 32-bit index arithmetic.
 // L lanes x 32 bytes cover a row chunk; 32/L neighbours per warp-wide load, U loads in flight per lane; 4 blocks of 256
-// threads per SM (64 registers); column chunks on blockIdx.y.  Sweep: profiles/r2_spmm_sweep*.log.
+// threads per SM (64 registers); column chunks on blockIdx.y.
 template <typename T, int L, int SCATTER>
 static int launch_v2(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst, int64_t dst_ld,
                      int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
@@ -134,12 +133,11 @@ static int launch_v2_sc(int sm_count, const CsrDev& A, int64_t n_rows, const T* 
 }
 
 // 64-byte rows (C = 16 floats / 8 doubles) with 32-byte lanes: two lanes per neighbour row, 8-lane row groups, two loads in
-// flight per lane — 0.267 ms against 0.337 ms for the 16-byte-lane kernel at N = 1M (profiles/r2_spmm_sweep_narrow_c16.log);
-// at C = 8 the 32-byte lanes bring nothing (0.20 vs 0.19 ms), those rows stay on spmm_hop_multirow_kernel.
+// flight per lane; rows of C = 8 stay on spmm_hop_multirow_kernel.
 template <typename T, int SCATTER>
 static int launch_multirow_v2(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst,
                               int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh = nullptr) {
-  constexpr int VEC = 32 / sizeof(T), L = 2, GS = 8, U = 2, THREADS = 256, MINB = sizeof(T) == 4 ? 4 : 3, HINT = 3;  // fp32: 4 blocks (0.266 ms) beat 3 (0.298 ms) although ptxas parks 16 bytes of per-row-group scalars on the stack
+  constexpr int VEC = 32 / sizeof(T), L = 2, GS = 8, U = 2, THREADS = 256, MINB = sizeof(T) == 4 ? 4 : 3, HINT = 3;
   auto kern = spmm_hop_multirow_v2_kernel<T, int32_t, VEC, L, GS, U, THREADS, MINB, HINT, SCATTER>;
   if (n_rows == 0) return B200GF_OK;
   constexpr int rows_per_block = (THREADS / 32) * (32 / GS);
@@ -263,7 +261,7 @@ int launch_bcast_rows(int dtype, const void* src, int64_t src_ld, int64_t n_rows
                       const BcastHost* bh) {
   if (!src || !bh || bh->n_peers <= 0 || bh->n_peers > MAX_PEERS || C <= 0 || src_ld < C || bh->out_ld < C) return B200GF_EINVAL;
   if (n_rows == 0) return B200GF_OK;
-  const int blocks = 148 * 8;
+  const int blocks = 132 * 8;
   if ((reinterpret_cast<uintptr_t>(src) & 15) || (reinterpret_cast<uintptr_t>(bh->mc) & 15)) return B200GF_EUNSUPPORTED;
   if (dtype == B200GF_F32) {
     if (C % 4 || src_ld % 4 || bh->out_ld % 4) return B200GF_EUNSUPPORTED;
@@ -296,7 +294,7 @@ int launch_scatter_rows(int dtype, const void* src, int64_t src_ld, int64_t n_ro
                         const ScatterHost* sh) {
   if (!src || !sh || sh->n_peers <= 0 || sh->n_peers > MAX_PEERS || C <= 0 || src_ld < C) return B200GF_EINVAL;
   if (n_rows == 0) return B200GF_OK;
-  const int blocks = 148 * 8;
+  const int blocks = 132 * 8;
   if (dtype == B200GF_F32) {
     if (C % 4 || src_ld % 4 || sh->gl % 4 || sh->out_ld % 4 || sh->out_col % 4 || sh->stride_b % 4) return B200GF_EUNSUPPORTED;
     scatter_rows_kernel<float, 4><<<blocks, 256, 0, st>>>((const float*)src, src_ld, n_rows, C, make_scatter<float>(sh));

@@ -2,7 +2,7 @@
 //
 //   dst[r, :] = sum_j A[r, j] * src[j, :]        A = CSR gather operator, src/dst node-major [rows, ld]
 //
-// Mapping (sm_100a, 148 SMs):
+// Mapping (sm_90a, 132 SMs):
 //   * one warp per (row, column chunk) work item, grid-stride over items in chunk-major order, so that at any
 //     time all resident warps gather from the same column slab (keeps it L2-resident when N * chunk_bytes fits);
 //   * L lanes x 16-byte vectors cover the chunk; the 32/L lane groups each take a different neighbour, so one
@@ -10,7 +10,7 @@
 //   * U independent LDG.128 per lane are in flight before the FMAs (memory-level parallelism);
 //   * col/val of a row are read once, coalesced (lane i holds entry i), and broadcast with SHFL;
 //   * PF (template flag, off in the library): prefetch of the next row's col/val and of the rowptr pair after it while
-//     the current row is gathered — measured slower (registers / issue slots), kept for the sweep tool.
+//     the current row is gathered — it costs registers and issue slots; kept for the sweep tool.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -29,7 +29,7 @@ struct Acc {
 
 // L2 cache policy: `frac` of the touched lines (chosen by address hash) get evict_last priority, the rest stay
 // evict_unchanged.  With the gathered feature matrix larger than the L2, a sticky subset that fits turns an LRU
-// thrash (measured 6 % L2 hit rate) into hits on that subset.
+// thrash into hits on that subset.
 __device__ __forceinline__ uint64_t evict_last_policy(float frac) {
   uint64_t pol;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, %1;" : "=l"(pol) : "f"(frac));
@@ -37,7 +37,7 @@ __device__ __forceinline__ uint64_t evict_last_policy(float frac) {
 }
 
 // HINT 0: ld.global.nc (default policy)   1: + L1::no_allocate (gathered rows have no L1 reuse)
-// HINT 2: L1::no_allocate + L2::evict_last on the gathered rows (fight for L2 residency of the feature slab)
+// HINT >= 2: L1::no_allocate + the L2 policy in `pol` on the gathered rows (fight for L2 residency of the feature slab)
 template <typename T, int VEC, int HINT>
 __device__ __forceinline__ Acc<T, VEC> load_vec(const T* p, uint64_t pol) {
   Acc<T, VEC> a;
@@ -54,35 +54,11 @@ __device__ __forceinline__ Acc<T, VEC> load_vec(const T* p, uint64_t pol) {
     }
     a.v[0] = t.x; a.v[1] = t.y; a.v[2] = t.z; a.v[3] = t.w;
   } else if constexpr (VEC * sizeof(T) == 32) {
-    // sm_100 256-bit load (LDG.E.256): one lane fetches a whole 32-byte sector.  HINT 0/1: L1::no_allocate only;
-    // HINT 3: L2::evict_last as a plain qualifier (no policy register); other HINTs: the policy in `pol`.
-    if constexpr (sizeof(T) == 4) {
-      unsigned r[8];
-      if constexpr (HINT == 3)
-        asm volatile("ld.global.nc.L1::no_allocate.L2::evict_last.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "l"(p));
-      else if constexpr (HINT >= 2)
-        asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8], %9;"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "l"(p), "l"(pol));
-      else
-        asm volatile("ld.global.nc.L1::no_allocate.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "l"(p));
+    // 32-byte lane: one lane covers a whole 32-byte sector with two adjacent 16-byte loads (sm_90 has no 256-bit load)
+    const Acc<T, VEC / 2> lo = load_vec<T, VEC / 2, HINT>(p, pol);
+    const Acc<T, VEC / 2> hi = load_vec<T, VEC / 2, HINT>(p + VEC / 2, pol);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) a.v[i] = __uint_as_float(r[i]);
-    } else {
-      double d[4];
-      if constexpr (HINT == 3)
-        asm volatile("ld.global.nc.L1::no_allocate.L2::evict_last.v4.b64 {%0,%1,%2,%3}, [%4];"
-                     : "=d"(d[0]), "=d"(d[1]), "=d"(d[2]), "=d"(d[3]) : "l"(p));
-      else if constexpr (HINT >= 2)
-        asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.b64 {%0,%1,%2,%3}, [%4], %5;"
-                     : "=d"(d[0]), "=d"(d[1]), "=d"(d[2]), "=d"(d[3]) : "l"(p), "l"(pol));
-      else
-        asm volatile("ld.global.nc.L1::no_allocate.v4.b64 {%0,%1,%2,%3}, [%4];"
-                     : "=d"(d[0]), "=d"(d[1]), "=d"(d[2]), "=d"(d[3]) : "l"(p));
-#pragma unroll
-      for (int i = 0; i < 4; ++i) a.v[i] = d[i];
-    }
+    for (int i = 0; i < VEC / 2; ++i) { a.v[i] = lo.v[i]; a.v[VEC / 2 + i] = hi.v[i]; }
   } else if constexpr (VEC == 2) {
     double2 t;
     if constexpr (HINT == 0) {
@@ -103,20 +79,13 @@ __device__ __forceinline__ Acc<T, VEC> load_vec(const T* p, uint64_t pol) {
 // SH 0: default store   1: st.global.cs (streaming: the result row is not re-read by this kernel)
 template <typename T, int VEC, int SH>
 __device__ __forceinline__ void store_vec(T* p, const Acc<T, VEC>& a) {
-  if constexpr (VEC * sizeof(T) == 32 && sizeof(T) == 4) {
-    // one 256-bit store per lane (STG.E.256): a row leaves as whole contiguous sectors — two 16-byte stores per lane
-    // would interleave half-sector writes across the warp, which costs on NVLink peer stores (fused all-gather epilogue)
-    if constexpr (SH == 1)
-      asm volatile("st.global.cs.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(a.v[0]), "f"(a.v[1]), "f"(a.v[2]),
-                   "f"(a.v[3]), "f"(a.v[4]), "f"(a.v[5]), "f"(a.v[6]), "f"(a.v[7]) : "memory");
-    else
-      asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(a.v[0]), "f"(a.v[1]), "f"(a.v[2]),
-                   "f"(a.v[3]), "f"(a.v[4]), "f"(a.v[5]), "f"(a.v[6]), "f"(a.v[7]) : "memory");
-  } else if constexpr (VEC * sizeof(T) == 32) {
-    if constexpr (SH == 1)
-      asm volatile("st.global.cs.v4.f64 [%0], {%1,%2,%3,%4};" ::"l"(p), "d"(a.v[0]), "d"(a.v[1]), "d"(a.v[2]), "d"(a.v[3]) : "memory");
-    else
-      asm volatile("st.global.v4.f64 [%0], {%1,%2,%3,%4};" ::"l"(p), "d"(a.v[0]), "d"(a.v[1]), "d"(a.v[2]), "d"(a.v[3]) : "memory");
+  if constexpr (VEC * sizeof(T) == 32) {
+    // 32-byte lane: two adjacent 16-byte stores
+    Acc<T, VEC / 2> lo, hi;
+#pragma unroll
+    for (int i = 0; i < VEC / 2; ++i) { lo.v[i] = a.v[i]; hi.v[i] = a.v[VEC / 2 + i]; }
+    store_vec<T, VEC / 2, SH>(p, lo);
+    store_vec<T, VEC / 2, SH>(p + VEC / 2, hi);
   } else if constexpr (VEC == 4) {
     if constexpr (SH == 1) __stcs(reinterpret_cast<float4*>(p), make_float4(a.v[0], a.v[1], a.v[2], a.v[3]));
     else *reinterpret_cast<float4*>(p) = make_float4(a.v[0], a.v[1], a.v[2], a.v[3]);
@@ -278,7 +247,7 @@ spmm_hop_kernel(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ 
 //     plain instantiation (SCATTER = false carries an empty struct).
 //
 // (2) A variant that stages the gathered rows in shared memory with cp.async and software-pipelines the index chain three
-//     units deep was built and measured (1.14-1.15 ms against 1.04 ms for (1), profiles/r2_spmm_sweep1_c64.log); it lives
+//     units deep was built and was slower than (1); it lives
 //     with the sweep tool (tools/spmm_async_variant.cuh), not in the library.
 // ---------------------------------------------------------------------------------------------------
 // Fused hop + all-gather (node-sharded multi-GPU path): the rank computes rows [row0, row0 + n_rows) of the next hop's
@@ -488,8 +457,7 @@ spmm_hop_multirow_v2_kernel(const IDX* __restrict__ rowptr, const int32_t* __res
 }
 
 // Narrow feature rows (C * sizeof(T) <= 128 bytes): one warp per row leaves most lanes idle and the kernel
-// latency-bound on the rowptr -> col/val -> gather dependency chain (measured 0.38 ms at C = 8 vs 1.27 ms at C = 64,
-// N = 1M).  Here a warp works on RPW = 32/GS consecutive rows at once: each group of GS lanes owns one row, reads
+// latency-bound on the rowptr -> col/val -> gather dependency chain.  Here a warp works on RPW = 32/GS consecutive rows at once: each group of GS lanes owns one row, reads
 // its col/val GS entries at a time, and its S = GS/L sub-groups of L lanes gather S neighbours per load.
 template <typename T, int VEC, int L, int GS, int U, int THREADS, int MINB, int HINT>
 __global__ void __launch_bounds__(THREADS, MINB)

@@ -3,7 +3,7 @@
 //   tap_grad     : dW_t = A^T · V_t                    — autograd of the above w.r.t. h (SURVEY.md §8 a-8)
 //   bias_grad    : db = column sums of dy
 //   pack_taps    : h[F,E,K,G] -> W[t][G][F] (t = 0 merges the k = 0 taps of every e, graphML.py:154)
-// The tcgen05 (3xTF32) contraction in tc_contract.cu takes over for the FP32 shapes it supports; these
+// The wgmma (3xTF32) contraction in tc_contract.cu takes over for the FP32 shapes it supports; these
 // kernels are the general path and the FP64 path.
 #include "common.cuh"
 
@@ -40,7 +40,7 @@ int launch_pack_taps(int dtype, const void* h, void* W, int F, int E, int K, int
   if (!h || !W || F <= 0 || E <= 0 || K <= 0 || G <= 0) return B200GF_EINVAL;
   const int64_t total = (int64_t)(1 + E * (K - 1)) * G * F;
   const int threads = 256;
-  const int blocks = (int)b200gf::imin64((total + threads - 1) / threads, 1184);
+  const int blocks = (int)b200gf::imin64((total + threads - 1) / threads, 132 * 8);
   if (dtype == B200GF_F32)
     pack_taps_kernel<float><<<blocks, threads, 0, st>>>((const float*)h, (float*)W, F, E, K, G, transpose_taps);
   else if (dtype == B200GF_F64)
@@ -142,7 +142,7 @@ int launch_tap_contract(int dtype, int64_t n_rows, int B, int P, int Q, int T, c
   if (dmma_contract_eligible(dtype, n_rows, B, P, Q, T, zs, z_ld, out, out_ld, accumulate)) {
     for (int t = 0; t < T; ++t)
       if (!zs[t] || z_ld[t] < (int64_t)B * P) return B200GF_EINVAL;
-    int sms = 148, dev = 0;                      // FP64: the DMMA kernel (dmma_contract.cu)
+    int sms = 132, dev = 0;                      // FP64: the DMMA kernel (dmma_contract.cu)
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     return launch_dmma_contract(sms, n_rows, B, P, Q, T, zs, z_ld, W, bias, bias_per_node, out, out_ld, st, act);
   }
@@ -189,7 +189,7 @@ static TapGradGeom tap_grad_geom(int64_t n_rows, int B, int P, int Q, int T) {
   g.q_tiles = (Q + TG_BQ - 1) / TG_BQ;
   const int64_t R = n_rows * B;
   const int64_t per = (int64_t)((T + 4) / 5) * g.p_tiles * g.q_tiles;  // the FP32 fast path groups 5 terms per block
-  int64_t want = (148 * 2 + per - 1) / per;  // aim at ~2 resident blocks per SM in total
+  int64_t want = (132 * 2 + per - 1) / per;  // aim at ~2 resident blocks per SM in total
   if (want < 1) want = 1;
   int64_t rpc = (R + want - 1) / want;
   if (rpc < 256) rpc = 256;
@@ -452,7 +452,7 @@ int launch_tap_grad(int dtype, int64_t n_rows, int B, int P, int Q, int T, const
     LAUNCH_CHECK();
   }
   const int64_t total = (int64_t)T * P * Q;
-  const int blocks = (int)b200gf::imin64((total + 255) / 256, 1184);
+  const int blocks = (int)b200gf::imin64((total + 255) / 256, 132 * 8);
   if (dtype == B200GF_F32)
     tap_grad_reduce_kernel<float><<<blocks, 256, 0, st>>>((const float*)scratch, g.n_chunks, T, P, Q, (float*)dW,
                                                           out_mode, E, K);
@@ -563,7 +563,7 @@ int launch_bias_grad(int dtype, int64_t n_rows, int B, int F, const void* dy, in
   if (bias_per_node) {
     const int64_t total = n_rows * F;
     if (total == 0) return B200GF_OK;
-    const int blocks = (int)b200gf::imin64((total + 255) / 256, 148 * 8);
+    const int blocks = (int)b200gf::imin64((total + 255) / 256, 132 * 8);
     if (dtype == B200GF_F32)
       bias_grad_node_kernel<float><<<blocks, 256, 0, st>>>((const float*)dy, dy_ld, n_rows, B, F, (float*)dbias);
     else
@@ -604,7 +604,7 @@ int b200gf_tap_contract(int dtype, int64_t n_rows, int B, int P, int Q, int T, c
   if (n_rows < 0 || B <= 0 || P <= 0 || Q <= 0 || T <= 0 || !zs || !z_ld || !W || !out) return B200GF_EINVAL;
   if (scratch && scratch_bytes >= tc_contract_scratch_bytes(T, P, Q) && (reinterpret_cast<uintptr_t>(scratch) & 15) == 0 &&
       tc_contract_eligible(dtype, n_rows, B, P, Q, T, zs, z_ld, out, out_ld, accumulate)) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     CUDA_TRY(cudaGetDevice(&dev));
     CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     int rc = launch_split_w(W, scratch, T, P, Q, (cudaStream_t)stream);

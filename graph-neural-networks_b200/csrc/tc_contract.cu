@@ -1,37 +1,36 @@
-// Tensor-core tap contraction for FP32 (sm_100a: TMA + tcgen05.mma kind::tf32 + TMEM), error-compensated ("3xTF32").
+// Tensor-core tap contraction for FP32 (sm_90a: TMA + wgmma tf32 + mbarrier), error-compensated ("3xTF32").
 //
 //   out[r, q] = bias[q] + sum_t sum_p Z_t[r, p] * W_t[p, q]          r = node * B + b
 //
 // replaces the reference's [B,N,EKG] x [EKG,F] torch.matmul + bias (alegnn/utils/graphML.py:170-175).
 // A single TF32 pass misses the 1e-4 tolerance over E*K*G = 320 terms (SURVEY.md §7 hard part 3), so every operand
-// is split x = hi + lo with hi = the 19 leading bits (exact in TF32) and the product is accumulated in FP32 in TMEM as
+// is split x = hi + lo with hi = the 19 leading bits (exact in TF32) and the product is accumulated in FP32 registers as
 //   hi*hi + lo*hi + hi*lo            (the dropped lo*lo term is ~2^-22 relative).
 //
-// One persistent CTA per SM, 320 threads, warp-specialised:
-//   warp 0        TMA producer: per 32-float k-chunk, one 128 x 32 tile of Z_t (128-byte swizzle) + the matching
-//                 Q x 32 tiles of W_hi and W_lo (pre-split, K-major) into a 4-stage shared-memory ring
-//   warps 2-5     splitter: writes lo = z - hi(z) next to the Z tile (same swizzled layout: the transform is
-//                 element-wise); the tile itself serves as the hi operand (the MMA truncates FP32 to TF32, which is
-//                 exactly hi), fence.proxy.async, then hands the stage to
-//   warp 1        MMA issuer: one elected lane issues 3 x 4 tcgen05.mma (M=128, N=Q, K=8) per stage into one of
-//                 two TMEM accumulators (so the epilogue of tile i overlaps the MMAs of tile i+1); tcgen05.commit
-//                 releases the stage to the producer and, after the last chunk, the accumulator to
-//   warps 6-9     epilogue: tcgen05.ld (32x32b), + bias, 16-byte stores of whole output rows.
+// One persistent CTA per SM, 384 threads = 3 warpgroups:
+//   warpgroup 0   TMA producer (one lane): per 32-float k-chunk, one 128 x 32 tile of Z_t (128-byte swizzle) + the
+//                 matching Q x 32 tiles of W_hi and W_lo (pre-split, K-major) into a shared-memory ring of stages
+//   warpgroups 1-2  consumers, 64 rows of the 128-row tile each: split their half of the Z tile in place (hi over the
+//                 tile, lo next to it; the transform is element-wise, so the swizzled layout does not matter),
+//                 fence.proxy.async, then 3 x 4 wgmma.m64nNk8 (N = Q rounded up to a power of two, the rows of W past Q
+//                 are never stored) per stage into FP32 register accumulators; the stage goes back to the producer once
+//                 the next stage's MMAs are issued (wgmma.wait_group 1), and the epilogue adds the bias, applies the
+//                 fused ReLU and stores the accumulators straight from registers.
 #include <cuda.h>
-
-#include <cstdlib>
 
 #include "common.cuh"
 
 namespace b200gf {
 namespace tc {
 
-constexpr int BM = 128;       // rows per tile  (UMMA M)
+constexpr int BM = 128;       // rows per tile (two warpgroups x wgmma M = 64)
 constexpr int BK = 32;        // floats per k-chunk = one 128-byte swizzle row
-constexpr int UMMA_K = 8;     // tf32: 32 bytes per instruction along K
+constexpr int MMA_K = 8;      // tf32: 32 bytes per instruction along K
 constexpr int MAX_T = 16;     // terms (tensor maps travel as kernel parameters)
-constexpr int THREADS = 320;
+constexpr int THREADS = 384;
 constexpr int A_BYTES = BM * BK * 4;  // 16 KB
+constexpr int HALF_BYTES = A_BYTES / 2;
+constexpr int SMEM_BUDGET = 200 * 1024;
 constexpr unsigned SPIN_LIMIT = 1u << 24;  // bounded waits: a protocol bug traps instead of hanging the GPU
 
 struct Params {
@@ -46,9 +45,6 @@ struct Params {
   int num_tiles;
   int stages;
   int bias_per_node;
-  int raw_hi;        // leave the TMA tile in place as the hi operand: the tensor core reads the top 19 bits of an FP32 value
-                     // (truncation), which IS hi — measured bit-identical to rewriting it (profiles/README.md), 16 KB less
-                     // shared-memory traffic per stage.  B200GF_TC_RAWHI=0 restores the rewrite.
   int relu;          // epilogue activation: out = max(out, 0)  (fused GraphFilter -> ReLU layer, architectures.py:287)
 };
 
@@ -84,67 +80,143 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint32_t bar
                ::"r"(dst), "l"(map), "r"(bar), "r"(x), "r"(y), "r"(z) : "memory");
 }
 
-// K-major, 128-byte-swizzled operand tile: 8-row groups 1024 bytes apart (SBO), LBO unused (=1), descriptor v1
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+// wgmma shared-memory descriptor of a K-major, 128-byte-swizzled operand tile: 8-row groups 1024 bytes apart (SBO),
+// LBO unused (=1), swizzle mode 1 (128 B) at bits 62-63.  Stepping along K inside the swizzle atom adds bytes to the start.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}"
-               ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, both from shared memory; N / 2 FP32 accumulators per thread
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t a, uint64_t b);
+template <>
+__device__ __forceinline__ void wgmma_tf32<16>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {"
+      "%0,%1,%2,%3,%4,%5,%6,%7"
+      "}, %8, %9, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(1));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15"
+      "}, %16, %17, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(1));
 }
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+      "}, %32, %33, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+      "}, %64, %65, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<256>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n .reg .pred p;\n setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+      "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+      "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+      "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,"
+      "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+      "}, %128, %129, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a), "l"(b), "r"(1));
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 __device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__float_as_uint(v) & 0xFFFFE000u); }
 
+__host__ __device__ constexpr int b_bytes(int NP) { return NP * BK * 4; }
+__host__ __device__ constexpr int stage_bytes(int NP) { return 2 * A_BYTES + 2 * b_bytes(NP); }
+
+// NP: the wgmma N, Q rounded up to a power of two (16 .. 256)
+template <int NP>
 __global__ void __launch_bounds__(THREADS, 1) tc_contract_kernel(const __grid_constant__ Params prm) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   // 1024-byte alignment for the 128-byte swizzle atoms
   unsigned char* smem = (unsigned char*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int Q = prm.Q;
+  constexpr int SB = stage_bytes(NP);
   const int S = prm.stages;
-  const int b_bytes = Q * BK * 4;
-  const int stage_bytes = 2 * A_BYTES + 2 * b_bytes;
-  unsigned char* bar_base = smem + (size_t)S * stage_bytes;
-  uint64_t* full = (uint64_t*)bar_base;            // [S] TMA landed
-  uint64_t* split = full + S;                      // [S] hi/lo written
-  uint64_t* empty = split + S;                     // [S] MMAs done with the stage
-  uint64_t* tmem_full = empty + S;                 // [2]
-  uint64_t* tmem_empty = tmem_full + 2;            // [2]
-  uint32_t* tmem_ptr = (uint32_t*)(tmem_empty + 2);
+  const int Q = prm.Q;
+  uint64_t* full = (uint64_t*)(smem + (size_t)S * SB);   // [S] TMA landed
+  uint64_t* empty = full + S;                            // [S] both consumers' MMAs done with the stage
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const int lane = threadIdx.x & 31;
   const int cpt = prm.P / BK;                      // k-chunks per term
   const int chunks = prm.T * cpt;
-  int tmem_cols = 32;
-  while (tmem_cols < 2 * Q) tmem_cols <<= 1;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(smem_u32(full + s), 1);
-      mbar_init(smem_u32(split + s), 128);
-      mbar_init(smem_u32(empty + s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(smem_u32(tmem_full + a), 1);
-      mbar_init(smem_u32(tmem_empty + a), 128);
+      mbar_init(smem_u32(empty + s), 8);           // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {  // TMEM allocation (whole warp), address lands in shared memory
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(tmem_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
+      const uint32_t tx = A_BYTES + 2 * Q * BK * 4;
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
         for (int t = 0; t < prm.T; ++t) {
@@ -152,129 +224,94 @@ __global__ void __launch_bounds__(THREADS, 1) tc_contract_kernel(const __grid_co
             const int s = it % S;
             const uint32_t ph = (it / S) & 1;
             mbar_wait(smem_u32(empty + s), ph ^ 1);
-            unsigned char* st = smem + (size_t)s * stage_bytes;
+            unsigned char* st = smem + (size_t)s * SB;
             const uint32_t bar = smem_u32(full + s);
-            mbar_expect_tx(bar, A_BYTES + 2 * b_bytes);
+            mbar_expect_tx(bar, tx);
             tma_load_2d(&prm.a_map[t], bar, smem_u32(st), pc * BK, tile * BM);
             tma_load_3d(&prm.bhi_map, bar, smem_u32(st + 2 * A_BYTES), pc * BK, 0, t);
-            tma_load_3d(&prm.blo_map, bar, smem_u32(st + 2 * A_BYTES + b_bytes), pc * BK, 0, t);
+            tma_load_3d(&prm.blo_map, bar, smem_u32(st + 2 * A_BYTES + b_bytes(NP)), pc * BK, 0, t);
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    // instruction descriptor: D=F32 (bit 4), A=B=TF32 (2 at bits 7 and 10), both K-major, N>>3 at 17, M>>4 at 24
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(Q >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-    uint32_t it = 0, tile_iter = 0;
-    for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x, ++tile_iter) {
-      const int a = tile_iter & 1;
-      const uint32_t aph = (tile_iter >> 1) & 1;
-      mbar_wait(smem_u32(tmem_empty + a), aph ^ 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t d_tmem = tmem_base + (uint32_t)(a * Q);
-      for (int c = 0; c < chunks; ++c, ++it) {
-        const int s = it % S;
-        const uint32_t ph = (it / S) & 1;
-        mbar_wait(smem_u32(split + s), ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (lane == 0) {
-          const uint32_t st = smem_u32(smem + (size_t)s * stage_bytes);
-#pragma unroll
-          for (int j = 0; j < BK / UMMA_K; ++j) {
-            const uint64_t a_hi = umma_desc(st + j * UMMA_K * 4);
-            const uint64_t a_lo = umma_desc(st + A_BYTES + j * UMMA_K * 4);
-            const uint64_t b_hi = umma_desc(st + 2 * A_BYTES + j * UMMA_K * 4);
-            const uint64_t b_lo = umma_desc(st + 2 * A_BYTES + b_bytes + j * UMMA_K * 4);
-            umma_tf32(d_tmem, a_hi, b_hi, idesc, (c > 0 || j > 0) ? 1u : 0u);
-            umma_tf32(d_tmem, a_lo, b_hi, idesc, 1u);
-            umma_tf32(d_tmem, a_hi, b_lo, idesc, 1u);
-          }
-          umma_commit(smem_u32(empty + s));                      // stage free once these MMAs retire
-          if (c == chunks - 1) umma_commit(smem_u32(tmem_full + a));  // accumulator complete
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 6) {
-    // ------------------------------------------------------------------ splitter (128 threads)
-    const int tid = threadIdx.x - 64;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
-      for (int c = 0; c < chunks; ++c, ++it) {
-        const int s = it % S;
-        const uint32_t ph = (it / S) & 1;
-        mbar_wait(smem_u32(full + s), ph);
-        float4* A = (float4*)(smem + (size_t)s * stage_bytes);
-        float4* Alo = (float4*)(smem + (size_t)s * stage_bytes + A_BYTES);
-#pragma unroll
-        for (int i = 0; i < A_BYTES / 16 / 128; ++i) {
-          const int idx = i * 128 + tid;
-          const float4 v = A[idx];
-          float4 hi, lo;
-          hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
-          lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
-          if (!prm.raw_hi) A[idx] = hi;
-          Alo[idx] = lo;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic writes -> visible to the tensor core
-        mbar_arrive(smem_u32(split + s));
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (128 threads)
-    const int q4 = warp & 3;  // TMEM lane quarter this warp may read
-    uint32_t tile_iter = 0;
-    for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x, ++tile_iter) {
-      const int a = tile_iter & 1;
-      const uint32_t aph = (tile_iter >> 1) & 1;
-      mbar_wait(smem_u32(tmem_full + a), aph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int64_t r = (int64_t)tile * BM + q4 * 32 + lane;
-      const bool row_ok = r < prm.R;
-      const int64_t n = row_ok ? r / prm.B : 0;
-      const int b = row_ok ? (int)(r - n * prm.B) : 0;
-      float* orow = prm.out + n * prm.out_ld + (int64_t)b * Q;
-      for (int c0 = 0; c0 < Q; c0 += 16) {
-        const uint32_t taddr = tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(a * Q + c0);
-        uint32_t v[16];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-              "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (row_ok) {
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            float4 o;
-            o.x = __uint_as_float(v[j]); o.y = __uint_as_float(v[j + 1]);
-            o.z = __uint_as_float(v[j + 2]); o.w = __uint_as_float(v[j + 3]);
-            if (prm.bias) {
-              const int q = c0 + j;
-              if (prm.bias_per_node) {
-                o.x += prm.bias[(int64_t)q * prm.n_rows + n]; o.y += prm.bias[(int64_t)(q + 1) * prm.n_rows + n];
-                o.z += prm.bias[(int64_t)(q + 2) * prm.n_rows + n]; o.w += prm.bias[(int64_t)(q + 3) * prm.n_rows + n];
-              } else {
-                o.x += __ldg(prm.bias + q); o.y += __ldg(prm.bias + q + 1);
-                o.z += __ldg(prm.bias + q + 2); o.w += __ldg(prm.bias + q + 3);
-              }
-            }
-            if (prm.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-            *reinterpret_cast<float4*>(orow + c0 + j) = o;
-          }
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(smem_u32(tmem_empty + a));
-    }
+    return;
   }
 
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols));
+  // -------------------------------------------------------------------- consumers (warpgroups 1 and 2)
+  const int h = wg - 1;                            // which 64-row half of the tile
+  const int tid = threadIdx.x & 127;
+  const int wq = tid >> 5;                         // warp within the warpgroup: rows 16 wq .. 16 wq + 15
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
+    float d[NP / 2];
+#pragma unroll
+    for (int i = 0; i < NP / 2; ++i) d[i] = 0.f;
+    for (int c = 0; c < chunks; ++c, ++it) {
+      const int s = it % S;
+      const uint32_t ph = (it / S) & 1;
+      mbar_wait(smem_u32(full + s), ph);
+      unsigned char* st = smem + (size_t)s * SB;
+      float4* A = (float4*)(st + h * HALF_BYTES);
+      float4* Alo = (float4*)(st + A_BYTES + h * HALF_BYTES);
+#pragma unroll
+      for (int i = 0; i < HALF_BYTES / 16 / 128; ++i) {
+        const int idx = i * 128 + tid;
+        const float4 v = A[idx];
+        float4 hi, lo;
+        hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
+        lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
+        A[idx] = hi;
+        Alo[idx] = lo;
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> visible to the tensor core
+      asm volatile("bar.sync %0, 128;" ::"r"(wg) : "memory");         // the whole half is split before any MMA reads it
+      const uint32_t sa = smem_u32(st);
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < BK / MMA_K; ++j) {
+        const uint64_t a_hi = gmma_desc(sa + h * HALF_BYTES + j * MMA_K * 4);
+        const uint64_t a_lo = gmma_desc(sa + A_BYTES + h * HALF_BYTES + j * MMA_K * 4);
+        const uint64_t b_hi = gmma_desc(sa + 2 * A_BYTES + j * MMA_K * 4);
+        const uint64_t b_lo = gmma_desc(sa + 2 * A_BYTES + b_bytes(NP) + j * MMA_K * 4);
+        wgmma_tf32<NP>(d, a_hi, b_hi);
+        wgmma_tf32<NP>(d, a_lo, b_hi);
+        wgmma_tf32<NP>(d, a_hi, b_lo);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                             // the previous stage's MMAs have retired: hand it back
+      if (c > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(empty + (it - 1) % S));
+      }
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(empty + (it - 1) % S));
+
+    // epilogue: accumulator d[4 n + 2 i + j] holds row 16 wq + lane / 4 + 8 i, column 8 n + 2 (lane % 4) + j
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int64_t r = (int64_t)tile * BM + h * 64 + wq * 16 + (lane >> 2) + 8 * i;
+      if (r >= prm.R) continue;
+      const int64_t n = r / prm.B;
+      const int b = (int)(r - n * prm.B);
+      float* orow = prm.out + n * prm.out_ld + (int64_t)b * Q;
+#pragma unroll
+      for (int nb = 0; nb < NP / 8; ++nb) {
+        const int q = nb * 8 + 2 * (lane & 3);
+        if (q >= Q) break;
+        float2 o = make_float2(d[4 * nb + 2 * i], d[4 * nb + 2 * i + 1]);
+        if (prm.bias) {
+          if (prm.bias_per_node) {
+            o.x += prm.bias[(int64_t)q * prm.n_rows + n]; o.y += prm.bias[(int64_t)(q + 1) * prm.n_rows + n];
+          } else {
+            o.x += __ldg(prm.bias + q); o.y += __ldg(prm.bias + q + 1);
+          }
+        }
+        if (prm.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+        *reinterpret_cast<float2*>(orow + q) = o;
+      }
+    }
   }
 }
 
@@ -340,11 +377,26 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
+// wgmma N for Q outputs: the next power of two (the B tile rows past Q are never stored)
+static int n_pad(int Q) {
+  int n = 16;
+  while (n < Q) n <<= 1;
+  return n;
+}
+
 static int stages_for(int Q) {
-  const int stage_bytes = 2 * A_BYTES + 2 * Q * BK * 4;
-  int s = (200 * 1024) / stage_bytes;
+  int s = SMEM_BUDGET / stage_bytes(n_pad(Q));
   if (s > 4) s = 4;
   return s;
+}
+
+template <int NP>
+static cudaError_t launch_np(const Params& prm, int grid, cudaStream_t st) {
+  const size_t smem = (size_t)prm.stages * stage_bytes(NP) + 1024 /*alignment slack*/ + 256 /*barriers*/;
+  cudaError_t e = cudaFuncSetAttribute(tc_contract_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  tc_contract_kernel<NP><<<grid, THREADS, smem, st>>>(prm);
+  return cudaSuccess;
 }
 
 }  // namespace tc
@@ -371,7 +423,7 @@ int launch_pack_taps_split(const void* h, void* whi_wlo, int F, int E, int K, in
   const int64_t total = (int64_t)(1 + E * (K - 1)) * G * F;
   float* hi = (float*)whi_wlo;
   float* lo = hi + total;
-  const int blocks = (int)imin64((total + 255) / 256, 1184);
+  const int blocks = (int)imin64((total + 255) / 256, 132 * 8);
   tc::pack_taps_split_kernel<<<blocks, 256, 0, st>>>((const float*)h, hi, lo, F, E, K, G, to_input);
   LAUNCH_CHECK();
   return B200GF_OK;
@@ -381,7 +433,7 @@ int launch_split_w(const void* W, void* whi_wlo, int T, int P, int Q, cudaStream
   const int64_t total = (int64_t)T * P * Q;
   float* hi = (float*)whi_wlo;
   float* lo = hi + total;
-  const int blocks = (int)imin64((total + 255) / 256, 1184);
+  const int blocks = (int)imin64((total + 255) / 256, 132 * 8);
   tc::split_w_kernel<<<blocks, 256, 0, st>>>((const float*)W, hi, lo, T, P, Q);
   LAUNCH_CHECK();
   return B200GF_OK;
@@ -431,15 +483,15 @@ int launch_tc_contract(int sm_count, int64_t n_rows, int B, int P, int Q, int T,
   prm.stages = stages_for(Q);
   prm.bias_per_node = bias_per_node;
   prm.relu = act;
-  {
-    static const int raw = [] { const char* e = getenv("B200GF_TC_RAWHI"); return (e && e[0] == '0') ? 0 : 1; }();
-    prm.raw_hi = raw;
-  }
-  const int stage_bytes = 2 * A_BYTES + 2 * Q * BK * 4;
-  const size_t smem = (size_t)prm.stages * stage_bytes + 1024 /*alignment slack*/ + 256 /*barriers*/;
-  CUDA_TRY(cudaFuncSetAttribute(tc_contract_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   const int grid = prm.num_tiles < sm_count ? prm.num_tiles : sm_count;
-  tc_contract_kernel<<<grid, THREADS, smem, st>>>(prm);
+  switch (n_pad(Q)) {
+    case 16: CUDA_TRY(launch_np<16>(prm, grid, st)); break;
+    case 32: CUDA_TRY(launch_np<32>(prm, grid, st)); break;
+    case 64: CUDA_TRY(launch_np<64>(prm, grid, st)); break;
+    case 128: CUDA_TRY(launch_np<128>(prm, grid, st)); break;
+    case 256: CUDA_TRY(launch_np<256>(prm, grid, st)); break;
+    default: return B200GF_EUNSUPPORTED;
+  }
   LAUNCH_CHECK();
   return B200GF_OK;
 }

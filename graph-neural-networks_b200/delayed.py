@@ -1,4 +1,4 @@
-"""Batch- and time-varying graph filter on the B200 LSIGF path (SURVEY.md §8f rank 4).
+"""Batch- and time-varying graph filter on the CUDA LSIGF path (SURVEY.md §8f rank 4).
 
     LSIGF_DB(h, S, x, b=None)                   <- alegnn/utils/graphML.py:977-1094
     GraphFilter_DB(G, F, K, E=1, bias=True)     <- graphML.py:3278-3393

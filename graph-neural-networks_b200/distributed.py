@@ -1,4 +1,4 @@
-"""Multi-GPU LSIGF (one process per GPU, torch.distributed over NCCL / NVLink 5) — SURVEY.md §8e.
+"""Multi-GPU LSIGF (one process per GPU, torch.distributed over NCCL / NVLink) — SURVEY.md §8e.
 
 Three shardings of  y = sum_{e,k} (x S_e^k) h_{e,k} + b  (each with its exchange fused into the hop kernel when the real
 CUDA ops run under NCCL, and with plain collectives otherwise — the variant the gloo tests exercise):
@@ -334,9 +334,8 @@ class PartitionedLSIGF:
         self.mode = mode
         self.symm_backend = symm_backend   # "auto": torch symmetric memory, else CUDA IPC; "ipc"; "torch"
         # all-gather epilogue: one multimem.st through the NVSwitch multicast address instead of P peer stores.  Off by
-        # default: measured slower for this pattern (2 GPUs: 2.78 vs 2.61 ms/step) — a multicast store also returns to the
-        # issuing GPU through its NVLink ingress, so every GPU receives N*C*s per hop instead of (P-1)/P of it, and the
-        # all-gather is ingress-bound (profiles/README.md)
+        # default: a multicast store also returns to the issuing GPU through its NVLink ingress, so every GPU receives
+        # N*C*s per hop instead of (P-1)/P of it, and the all-gather is ingress-bound
         self.multicast = bool(multicast)
         self.fence = fence          # "flags": peer flags in symmetric memory (no NCCL at all); "nccl": 4-byte all-reduce
         # fused = hop kernels scatter their rows over NVLink themselves (no NCCL collective on the data path);

@@ -4,7 +4,7 @@ The reference's recurrent layers issue one small LSIGF per time step (graphML.py
 a handful of microsecond kernels, so a sequence of T steps is bound by launch latency and Python, not by the GPU.  Every
 kernel of this library is enqueued on the caller's stream without host synchronisation or allocation
 (include/b200gf.h) — so the complete T-step recursion, filters, gates and non-linearities included, can be captured once
-and replayed as ONE graph launch (measured: 2.2-2.4x on a 40-step sequence, profiles/README.md).
+and replayed as ONE graph launch.
 
     run = gnn_b200.graphed(layer, x_example, z0_example)      # warm-up + capture (inference: no autograd inside)
     z, zT = run(x, z0)                                        # copies into the static inputs, replays, returns the

@@ -1,4 +1,4 @@
-"""Static-GSO graph recurrent layers on top of the B200 LSIGF path (SURVEY.md §8f rank 2).
+"""Static-GSO graph recurrent layers on top of the CUDA LSIGF path (SURVEY.md §8f rank 2).
 
     GatedGRNN(a, b, S, x, z0, sigma, q_hat, q_check, xBias, zBias)   <- alegnn/utils/graphML.py:1292-1527
     HiddenState(F, H, K, nonlinearity, E, bias)                       <- graphML.py:3540-3681
@@ -211,7 +211,9 @@ class _GatedHiddenState(HiddenState):
 
     def addGSO(self, S):
         HiddenState.addGSO(self, S)
-        self._make_gate_maps()                      # fresh gate maps on every addGSO, as in the reference
+        # fresh gate maps on every addGSO, as in the reference; initialised as the reference does, then placed on the
+        # layer's device (a layer moved to the GPU before addGSO keeps its gates there too)
+        self._make_gate_maps()
         self.inputGateGRNN.addGSO(S)
         self.forgetGateGRNN.addGSO(S)
 
@@ -220,8 +222,9 @@ class TimeGatedHiddenState(_GatedHiddenState):
     """graphML.py:3683-3855: one scalar gate per (sample, time step): q = sigmoid(Linear(H*N -> 1)(z_gate[b, t]))."""
 
     def _make_gate_maps(self):
-        self.inputGateFC = nn.Linear(self.H * self.N, 1, self.bias)       # graphML.py:3838-3839
-        self.forgetGateFC = nn.Linear(self.H * self.N, 1, self.bias)
+        dev = self.aWeights.device
+        self.inputGateFC = nn.Linear(self.H * self.N, 1, self.bias).to(dev)       # graphML.py:3838-3839
+        self.forgetGateFC = nn.Linear(self.H * self.N, 1, self.bias).to(dev)
 
     def _gates(self, x, z0):
         B, T = x.shape[0], x.shape[1]
@@ -237,8 +240,9 @@ class NodeGatedHiddenState(_GatedHiddenState):
     """graphML.py:3857-4031: one gate per (sample, time step, node): q = sigmoid(GraphFilter(H -> 1)(z_gate))."""
 
     def _make_gate_maps(self):
-        self.inputGateGraphFilter = _gml.GraphFilter(self.H, 1, self.K, bias=self.bias)   # graphML.py:4008-4009
-        self.forgetGateGraphFilter = _gml.GraphFilter(self.H, 1, self.K, bias=self.bias)
+        dev = self.aWeights.device
+        self.inputGateGraphFilter = _gml.GraphFilter(self.H, 1, self.K, bias=self.bias).to(dev)   # graphML.py:4008-4009
+        self.forgetGateGraphFilter = _gml.GraphFilter(self.H, 1, self.K, bias=self.bias).to(dev)
         self.inputGateGraphFilter.addGSO(self.S)
         self.forgetGateGraphFilter.addGSO(self.S)
 

@@ -1,5 +1,5 @@
 /*
- * b200gf — C ABI of the B200-native LSIGF graph-filter path.
+ * b200gf — C ABI of the H100-native LSIGF graph-filter path.
  *
  * This is the drop-in boundary for ONE path of alelab-upenn/graph-neural-networks (alegnn 0.4.0):
  *
@@ -50,7 +50,7 @@ enum {
   B200GF_EUNSUPPORTED = -2,/* dtype / size not supported                                           */
   B200GF_ENOMEM = -3,      /* host or device allocation failed in plan_create                      */
   B200GF_EWORKSPACE = -4,  /* workspace smaller than b200gf_workspace_bytes()                      */
-  B200GF_ENODEVICE = -5,   /* no CUDA device / wrong architecture (needs sm_100)                   */
+  B200GF_ENODEVICE = -5,   /* no CUDA device / wrong architecture (needs sm_90)                    */
   B200GF_ECUDA = -1000     /* -(1000 + cudaError_t)                                                */
 };
 
@@ -243,7 +243,7 @@ int b200gf_peer_wait(const void* my_flags, int n_peers, const void* local_step, 
  * bias NULL / [Q] / [Q, n_rows] (bias_per_node).  accumulate != 0 adds to the existing `out`.
  * scratch (optional, b200gf_tap_contract_scratch_bytes(T,P,Q) bytes, 16-byte aligned): when given, FP32 problems
  * with P % 32 == 0, Q % 16 == 0, Q <= 256, T <= 16, z_ld == B*P and accumulate == 0 run on the tensor cores
- * (tcgen05 kind::tf32 with hi/lo error compensation, "3xTF32"); everything else uses the FP32/FP64 FMA kernel. */
+ * (wgmma tf32 with hi/lo error compensation, "3xTF32"); everything else uses the FP32/FP64 FMA kernel. */
 int b200gf_tap_contract(int dtype, int64_t n_rows, int B, int P, int Q, int T,
                         const void* const* zs, const int64_t* z_ld, const void* W,
                         const void* bias, int bias_per_node,

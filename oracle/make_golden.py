@@ -1,7 +1,7 @@
-"""Generate tests/golden/*.npz by running the UNMODIFIED reference (alegnn) in this container.
+"""Generate tests/golden/*.npz by running the UNMODIFIED reference (alegnn).
 
-TEST INFRASTRUCTURE.  Run once here (`python oracle/make_golden.py`); the fixtures are committed because
-/root/reference does not exist on the GPU box.  Every array in a fixture is either a seeded input or an
+TEST INFRASTRUCTURE.  Run once (`B200GF_REFERENCE_ROOT=<alegnn checkout> python oracle/make_golden.py`); the fixtures are
+committed so that the tests need no reference checkout.  Every array in a fixture is either a seeded input or an
 output of the reference's own code:
 
   lsigf_cases.npz   – `alegnn.utils.graphML.LSIGF` (graphML.py:83-176) forward in fp64 and its autograd

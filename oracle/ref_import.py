@@ -1,7 +1,8 @@
-"""Import the UNMODIFIED reference (`alegnn`) from /root/reference for fixture generation.
+"""Import the UNMODIFIED reference (`alegnn`) for fixture generation.
 
-TEST INFRASTRUCTURE ONLY.  Used by `oracle/make_golden.py` (and by tests that are skipped when
-/root/reference is absent, i.e. on the GPU box).  Nothing in the product path imports this.
+TEST INFRASTRUCTURE ONLY.  B200GF_REFERENCE_ROOT names the directory of an alegnn checkout (the one holding `alegnn/`).
+Used by `oracle/make_golden.py` and by the recording mode of oracle/ref_golden.py; the tests themselves read the stored
+results and need no checkout.  Nothing in the product path imports this.
 
 The reference pulls optional plotting / dataset packages at import time
 (`alegnn/utils/graphTools.py:40-43`, `alegnn/utils/dataTools.py:33,38-43,4335`); they are not on the
@@ -13,17 +14,17 @@ import sys
 import types
 from unittest import mock
 
-REFERENCE_ROOT = os.environ.get("B200GF_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("B200GF_REFERENCE_ROOT", "")
 
 
 def reference_available():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "alegnn"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "alegnn"))
 
 
 def import_reference():
     """Returns the reference module `alegnn.utils.graphML` (and makes `alegnn` importable)."""
     if not reference_available():
-        raise ImportError("reference tree not present at %s" % REFERENCE_ROOT)
+        raise ImportError("reference tree not present (set B200GF_REFERENCE_ROOT): %r" % REFERENCE_ROOT)
     import numpy as np
     if not hasattr(np, "int"):
         np.int = int

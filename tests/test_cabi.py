@@ -195,7 +195,7 @@ def test_layout_and_tap_blocks():
     (50000, 1, 64, 64, 5, "q"),       # several tiles per CTA: accumulator double-buffering and ring wrap-around
 ])
 def test_tensor_core_tap_contract(N, B, P, Q, T, bias_mode):
-    """tcgen05 3xTF32 contraction (tc_contract.cu) vs an fp64 einsum; must sit at FP32 accuracy, far inside 1e-4."""
+    """wgmma 3xTF32 contraction (tc_contract.cu) vs an fp64 einsum; must sit at FP32 accuracy, far inside 1e-4."""
     import gnn_b200
     cabi = gnn_b200._cabi
     lib = cabi.load()

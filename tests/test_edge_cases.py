@@ -175,3 +175,24 @@ def test_plan_cache_follows_in_place_gso_updates():
                           x.cpu().double().numpy(), layer.bias.detach().cpu().double().numpy())
     assert _rel(y1.detach().cpu().numpy(), ref) < 1e-5
     assert not torch.allclose(y0, y1)
+
+
+@pytest.mark.gpu
+def test_host_taps_or_bias_are_rejected():
+    """The kernels read h and b on the device: host tensors must raise before any launch, not reach a kernel as host
+    pointers.  A node-gated layer moved to the GPU before addGSO builds its gate filters on the GPU as well."""
+    import gnn_b200
+    from gnn_b200 import recurrent as rec
+    c = orc.random_case(13, N=30, B=2, G=3, F=4, K=3, E=1, avg_deg=4, bias="F1")
+    gpu = lambda a: torch.tensor(a, dtype=torch.float32, device="cuda")  # noqa: E731
+    cpu = lambda a: torch.tensor(a, dtype=torch.float32)  # noqa: E731
+    with pytest.raises(RuntimeError, match="on one device"):
+        gnn_b200.LSIGF(cpu(c["h"]), gpu(c["S"]), gpu(c["x"]), gpu(c["b"]))
+    with pytest.raises(RuntimeError, match="on one device"):
+        gnn_b200.LSIGF(gpu(c["h"]), gpu(c["S"]), gpu(c["x"]), cpu(c["b"]))
+    layer = rec.NodeGatedHiddenState(2, 4, 3).cuda()
+    layer.addGSO(gpu(c["S"]))
+    assert all(p.is_cuda for p in layer.parameters())
+    z, _ = layer(torch.randn(2, 3, 2, 30, device="cuda"), torch.randn(2, 4, 30, device="cuda"))
+    torch.cuda.synchronize()
+    assert z.shape == (2, 3, 4, 30) and bool(torch.isfinite(z).all())

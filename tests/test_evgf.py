@@ -59,7 +59,7 @@ def test_evgf_functional_gpu(z, dtype, tol):
 @pytest.mark.parametrize("dtype,tol", [(torch.float64, 1e-11), (torch.float32, 1e-4)])
 def test_edge_variant_layer_gpu(z, tag, dtype, tol):
     """Reference parameter names/shapes load as a state_dict; output, dx and every parameter gradient match the
-    reference layer (hybrid: LSI part through the B200 LSIGF, bias counted twice as in graphML.py:2682,2686)."""
+    reference layer (hybrid: LSI part through the CUDA LSIGF, bias counted twice as in graphML.py:2682,2686)."""
     import gnn_b200
     N, M, E, K, G, F, B, Nin = [int(v) for v in z[tag + "_meta"]]
     layer = gnn_b200.EdgeVariantGF(G, F, K, M, N, E, True).to("cuda", dtype)

@@ -98,7 +98,7 @@ def test_fused_layer_golden_gpu(golden_dir, dtype, tol, fuse):
 
 @pytest.mark.gpu
 def test_fused_relu_on_the_tensor_core_contraction():
-    """G = F = 64 takes the tcgen05 contraction: its epilogue applies the ReLU; backward masks with the saved output."""
+    """G = F = 64 takes the wgmma contraction: its epilogue applies the ReLU; backward masks with the saved output."""
     import gnn_b200
     from gnn_b200 import graphs
     N, K, G, F, B = 30000, 4, 64, 64, 2

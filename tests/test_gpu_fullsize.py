@@ -1,4 +1,4 @@
-"""Oracle parity at BASELINE.json's FULL sizes (`pytest -m gpu`, B200 box): the CUDA path vs the fp64 CPU oracle on
+"""Oracle parity at BASELINE.json's FULL sizes (`pytest -m gpu`, H100): the CUDA path vs the fp64 CPU oracle on
 random inputs with all feature columns distinct — forward and every gradient.  VERDICT r1 "weak #1": the earlier
 full-size test only compared the CUDA path with itself (fixed point / linearity / adjoints).
 

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: `pytest -m gpu`): the CUDA path behind the C ABI vs
+"""GPU parity tests (run on an H100: `pytest -m gpu`): the CUDA path behind the C ABI vs
   (1) golden fixtures produced by the UNMODIFIED reference (tests/golden, oracle/make_golden.py),
   (2) the fp64 CPU oracle (oracle/lsigf_oracle.py) on seeded sparse graphs the dense reference could not hold,
   (3) size-independent properties at BASELINE.json's full sizes.
@@ -224,7 +224,7 @@ def test_full_size_properties(b200, N, deg):
 
 def test_forward_is_cuda_graph_capturable(b200):
     """include/b200gf.h promises no allocation and no host synchronisation inside b200gf_forward: capture one call
-    (hops + tcgen05 contraction) in a CUDA graph, replay it on new input values, compare with an eager call."""
+    (hops + wgmma contraction) in a CUDA graph, replay it on new input values, compare with an eager call."""
     from gnn_b200 import graphs, _cabi
     lib = _cabi.load()
     N, K, G, F, B = 20000, 4, 64, 64, 1

@@ -2,7 +2,7 @@
 unmodified reference (tests/golden/lsigf_db_cases.npz <- oracle/make_golden.py gen_lsigf_db; graphML.py:977-1094,
 :3278-3393).
 
-The B200 path folds the B*T per-sample graphs into one space-time sparse operator and runs the ordinary LSIGF kernels
+The CUDA path folds the B*T per-sample graphs into one space-time sparse operator and runs the ordinary LSIGF kernels
 on it.  CPU tests check that construction (CSR layout, delay / zero-history semantics, bias tiling, autograd wiring)
 with the dense CPU oracle applied to the same CSR; GPU tests run it through the CUDA filter."""
 import os

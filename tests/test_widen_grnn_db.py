@@ -2,7 +2,7 @@
 produced by the unmodified reference (tests/golden/grnn_db_cases.npz <- oracle/make_golden.py gen_grnn_db;
 graphML.py:1096-1290, :3395-3538).
 
-The B200 path keeps the K-1 delayed copies of the hidden state node-major and advances them with one CSR hop per time step
+The CUDA path keeps the K-1 delayed copies of the hidden state node-major and advances them with one CSR hop per time step
 and edge feature (operator (t, e) of ONE device plan built from the GSO batch).  CPU tests check the operator construction
 and the recursion / autograd wiring with torch.sparse standing in for the hop kernel and the dense CPU oracle for the
 input-to-hidden filter; GPU tests run the same fixtures through the CUDA kernels."""

@@ -1,4 +1,4 @@
-"""Runs a few LSIGF forward+backward steps on the headline workload (for `ncu` launch lists of the backward pass)."""
+"""Runs a few LSIGF forward+backward steps on the headline workload (for a profiler's launch list of the backward pass)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

@@ -1,5 +1,5 @@
-// cp.async-staged variant of the hop kernel — measured in round 2 (profiles/r2_spmm_sweep1_c64.log: 1.14-1.15 ms per hop
-// against 1.04 ms for the shipped spmm_hop_v2_kernel), kept with the sweep tool as the evidence for DESIGN.md §3.1.
+// cp.async-staged variant of the hop kernel — it was slower than the shipped spmm_hop_v2_kernel and is kept with the sweep
+// tool as an alternative to re-measure (DESIGN.md §3.1).
 //
 // Gathered rows are staged in shared memory with cp.async (LDGSTS.128, L2-only), so the number of bytes in flight per SM
 // is set by shared memory (2 x SLOTS neighbour rows per warp) instead of by registers, and the index chain

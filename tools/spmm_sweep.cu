@@ -1,8 +1,8 @@
 // Tuning sweep for the hop kernel (spmm_kernels.cuh) on a synthetic random graph.  Not part of the library.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 tools/spmm_sweep.cu -o tools/spmm_sweep
-//   tools/spmm_sweep [N=1000000] [deg=32] [C=64] [reps=10] [peakGBs=6566.7]
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 tools/spmm_sweep.cu -o tools/spmm_sweep
+//   tools/spmm_sweep [N=1000000] [deg=32] [C=64] [reps=10] [peakGBs=3350 (H100 SXM data sheet)]
 // Prints one line per variant: registers, resident blocks/SM, ms per hop, algorithmic GB/s (gather model,
-// SURVEY.md §8d) and the fraction of the measured HBM copy bandwidth.
+// SURVEY.md §8d) and the fraction of the given HBM bandwidth.
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -208,7 +208,7 @@ int main(int argc, char** argv) {
   const int deg = argc > 2 ? atoi(argv[2]) : 32;
   const int C = argc > 3 ? atoi(argv[3]) : 64;
   const int reps = argc > 4 ? atoi(argv[4]) : 10;
-  const double peak = argc > 5 ? atof(argv[5]) : 6566.7;
+  const double peak = argc > 5 ? atof(argv[5]) : 3350.0;
   cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, 0));
   printf("device %s  SMs %d  N=%lld deg=%d C=%d\n", prop.name, prop.multiProcessorCount, (long long)N, deg, C);
   printf("L2 %d MB, persistingL2CacheMaxSize %d MB, accessPolicyMaxWindowSize %d MB\n", prop.l2CacheSize >> 20,
