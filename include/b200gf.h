@@ -171,7 +171,10 @@ int b200gf_profile_read(b200gf_plan* plan, float* ms, int n);
  * ---------------------------------------------------------------------------------------------- */
 
 /* one shift: dst[r, 0:C] = sum_j A_e[r, j] src[j, 0:C] for the plan's n_rows rows; A = S_e^T (FWD) or S_e (BWD).
- * src has n_cols rows of stride src_ld, dst has n_rows rows of stride dst_ld. */
+ * src has n_cols rows of stride src_ld, dst has n_rows rows of stride dst_ld.  The vector kernels load and store whole
+ * 16- or 32-byte vectors, so they read src[j, C : min(src_ld, padded)) and may write dst[r, C : min(dst_ld, padded)),
+ * padded = C rounded up to 32 bytes (8 floats / 4 doubles); those dst columns hold no meaningful value afterwards.
+ * Nothing at or past that column, and no row at or past n_rows, is written. */
 int b200gf_hop(const b200gf_plan* plan, int e, int direction,
                const void* src, int64_t src_ld, void* dst, int64_t dst_ld, int C, void* stream);
 
