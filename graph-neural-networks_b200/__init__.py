@@ -11,6 +11,7 @@ from .edgevariant import EVGF, EdgeVariantGF, SparseEdgeVariantGF  # noqa: F401,
 from .pooling import MaxPoolLocal  # noqa: F401,E402
 from .activations import MaxLocalActivation, MedianLocalActivation, NoActivation  # noqa: F401,E402
 from .recurrent import GatedGRNN, HiddenState, TimeGatedHiddenState, NodeGatedHiddenState  # noqa: F401,E402
+from .edgegated import EdgeGatedGRNN, EdgeGatedHiddenState, EdgeGatePattern  # noqa: F401,E402
 from .delayed import LSIGF_DB, GraphFilter_DB, GRNN_DB, HiddenState_DB  # noqa: F401,E402
 from .graphed import graphed, GraphedForward  # noqa: F401,E402
 

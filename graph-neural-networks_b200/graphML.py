@@ -323,15 +323,16 @@ def fuse_layers(model):
 _SAVED = {}
 
 
-def install(gml=None):
+def install(gml=None, edge_gating=False):
     """Point `alegnn.utils.graphML.LSIGF`, `.GraphFilter`, `.EVGF`, `.EdgeVariantGF`, the local pooling / activation
-    layers and the static-GSO recurrent layers at this package.
+    layers and the static-GSO recurrent layers at this package.  `edge_gating=True` also points
+    `.EdgeGatedHiddenState` at the sparse edge-gated layer (edgegated.py); by default it stays the reference's.
 
     `GraphFilter.forward` in the reference looks `LSIGF` up as a module global at call time (graphML.py:2137), so
     this also accelerates its hybrid EdgeVariantGF (:2686), jARMA (:592) and GatedGRNN (:1403,:1461) call sites.
     Architectures built AFTER install() get this package's layers (plan cached in addGSO).
     """
-    from . import activations, delayed, edgevariant, pooling, recurrent
+    from . import activations, delayed, edgegated, edgevariant, pooling, recurrent
     if gml is None:
         import alegnn.utils.graphML as gml
     if id(gml) not in _SAVED:
@@ -341,6 +342,10 @@ def install(gml=None):
                                                              "TimeGatedHiddenState", "NodeGatedHiddenState",
                                                              "LSIGF_DB", "GraphFilter_DB", "GRNN_DB",
                                                              "HiddenState_DB")})
+    if edge_gating:
+        _SAVED[id(gml)][1].setdefault("EdgeGatedHiddenState", getattr(gml, "EdgeGatedHiddenState"))
+        # per-non-zero attention gates and the per-sample gated hop (edgegated.py); gml.GatedGRNN stays the reference's
+        gml.EdgeGatedHiddenState = edgegated.EdgeGatedHiddenState
     gml.LSIGF = LSIGF
     gml.GraphFilter = GraphFilter
     gml.EVGF = edgevariant.EVGF

@@ -19,7 +19,7 @@ here is the data movement between them:
     GraphRecurrentNN.splitForward (architectures.py:4551) is again a node-major view the output filter consumes in place.
 
 Edge gating (5-D gates, graphML.py:1410-1451 / :1474-1514) multiplies a dense N x N gate into the GSO per sample and
-time step — that is the batch-/time-varying-GSO path (LSIGF_DB family, §8f rank 4) and is not provided here: it raises.
+time step; it runs on per-non-zero gates in edgegated.py (EdgeGatedGRNN / EdgeGatedHiddenState), and GatedGRNN raises.
 """
 import math
 
@@ -44,7 +44,8 @@ def _check_gate(q, B, T, N, name):
     if q.dim() > 4:
         raise NotImplementedError(
             "b200gf: edge gating (%s of shape %s) needs a per-sample, per-time-step GSO (graphML.py:1410-1451); "
-            "only ungated, time-gated and node-gated recursions run on the static-GSO path" % (name, tuple(q.shape)))
+            "only ungated, time-gated and node-gated recursions run on the static-GSO path; edge-gated recursions run on "
+            "per-non-zero gates in gnn_b200.EdgeGatedGRNN / EdgeGatedHiddenState" % (name, tuple(q.shape)))
     assert q.dim() == 4
     assert q.shape[1] == T
     assert q.shape[2] == 1

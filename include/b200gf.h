@@ -285,6 +285,46 @@ int b200gf_ev_backward(int dtype, int64_t NA, int B, int G, int F, int K,
                        const void* w, const void* xT, const void* states, const void* dY,
                        void* lam, void* dw, void* dxT, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Edge-gated recurrent layer (EdgeGatedHiddenState, alegnn/utils/graphML.py:4033-4209; E = 1): the reference's dense
+ * B*T x N x N attention gates (learnAttentionGSO, :640-737) kept per non-zero of the mask |S + I| > 1e-9, and the hop
+ * with a different gated GSO per sample (GatedGRNN's edge path, :1410-1451, :1474-1514).  Bs = number of samples.
+ *   mask CSR: rowptr [N+1], col [nnz] (columns ascending); its transpose: rowptrT [N+1], permT [nnz] = position in the
+ *   mask CSR of the k-th entry of column j.  s, dsig1, dsig2: [N, Bs]; alpha, dalpha, dlogit: [nnz, Bs] (sample
+ *   innermost).  mixer: DEVICE pointer to the two mixer values (a1, a2).
+ *
+ * attention forward: alpha[q, b] = softmax over the mask row i of LeakyReLU_0.2(a1 s[j, b] + a2 s[i, b]), q = (i, j).
+ * attention backward: dlogit = the softmax and LeakyReLU backward of dalpha (scratch, [nnz, Bs]);
+ *   dsig2[i, b] = sum over row i of dlogit, dsig1[j, b] = sum over column j of dlogit (gather over the transpose);
+ *   ds = a1 dsig1 + a2 dsig2, da1 = sum s dsig1, da2 = sum s dsig2 are left to the caller.
+ * gated hop forward: dst[j, b*C + c] = sum_i S_ij gate[b, p(i, j)] src[i, b*C + c] over the CSR of S^T (rowptrT, colT,
+ *   valT) with posT = p(i, j), the entry's position in the mask CSR (-1: outside the mask, contributes nothing).
+ *   gate[b, p] is read at gate + b*gate_sb + p*gate_sp.  src / dst node-major, ld >= Bs*C.
+ * gated hop backward: dsrc (NULL to skip) = the same hop over the CSR of S (rowptr, col, val, pos) applied to ddst;
+ *   dgate (NULL to skip) [b, q] = m_sval[q] * sum_c src[i, b*C + c] ddst[j, b*C + c] for EVERY mask entry q = (i, j),
+ *   m_sval [nnz] = S_ij in mask order (0 where S has no entry), written at dgate + b*dgate_sb + q*dgate_sp.
+ * All four are deterministic (one writer per output element, fixed summation order).
+ * ---------------------------------------------------------------------------------------------- */
+int b200gf_egate_attention_forward(int dtype, int64_t N, int64_t nnz, int Bs,
+                                   const int64_t* rowptr, const int32_t* col,
+                                   const void* s, const void* mixer, void* alpha, void* stream);
+int b200gf_egate_attention_backward(int dtype, int64_t N, int64_t nnz, int Bs,
+                                    const int64_t* rowptr, const int32_t* col,
+                                    const int64_t* rowptrT, const int32_t* permT,
+                                    const void* s, const void* mixer, const void* alpha, const void* dalpha,
+                                    void* dlogit, void* dsig1, void* dsig2, void* stream);
+int b200gf_gated_hop_forward(int dtype, int64_t N, int Bs, int C,
+                             const int64_t* rowptrT, const int32_t* colT, const void* valT, const int32_t* posT,
+                             const void* gate, int64_t gate_sb, int64_t gate_sp,
+                             const void* src, int64_t src_ld, void* dst, int64_t dst_ld, void* stream);
+int b200gf_gated_hop_backward(int dtype, int64_t N, int Bs, int C,
+                              const int64_t* rowptr, const int32_t* col, const void* val, const int32_t* pos,
+                              const int64_t* m_rowptr, const int32_t* m_col, const void* m_sval,
+                              const void* gate, int64_t gate_sb, int64_t gate_sp,
+                              const void* src, int64_t src_ld, const void* ddst, int64_t ddst_ld,
+                              void* dsrc, int64_t dsrc_ld, void* dgate, int64_t dgate_sb, int64_t dgate_sp,
+                              void* stream);
+
 /* layout conversion between the reference's [C, N] (feature-major, C = B*G) and node-major [N, ld] */
 int b200gf_to_node_major(int dtype, const void* src_cn, void* dst_nc, int64_t dst_ld,
                          int64_t N, int C, void* stream);
