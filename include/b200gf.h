@@ -275,6 +275,8 @@ size_t b200gf_tap_grad_scratch_bytes(int dtype, int64_t n_rows, int B, int P, in
  * forward : n_states >= K-1 keeps u_0 .. u_{K-2} for the backward pass; n_states == 2 ping-pongs (inference).
  * backward: dY [F, NA, B] -> dw [F, K, G, nnz], dxT [G, NA, B]; needs the transposed pattern (rowptrT, colT) with
  *           perm[it] = index of that entry in the forward pattern, and lam = scratch of 2 * F*G*NA*B elements.
+ *           Every element of dw is written, so it need not be zeroed first; with diag, the k = 0 slots other than
+ *           the diagonal ones (and every k = 0 slot of a row with diag[i] = -1) are written with exactly 0.
  * ---------------------------------------------------------------------------------------------- */
 int b200gf_ev_forward(int dtype, int64_t NA, int B, int G, int F, int K,
                       const int64_t* rowptr, const int32_t* col, const int32_t* diag, int64_t nnz,

@@ -195,11 +195,36 @@ def test_sparse_edge_variant_layer_gpu(z, tag, dtype, tol):
     _check_sparse_layer(z, tag, layer, dims, dtype, "cuda", tol)
 
 
+def _twin_fp64(layer, gso, x, dy, absolute):
+    """The fp32 layer's parameters and inputs cast to fp64 (absolute values when `absolute`: the run that gives the
+    magnitudes M of the error envelope) through the same kernels -> (y, x.grad, [weightEV[e].grad])."""
+    import gnn_b200
+    f = (lambda t: t.detach().double().abs()) if absolute else (lambda t: t.detach().double())   # noqa: E731
+    g64 = gso.astype(torch.float64)
+    if absolute:
+        g64 = gnn_b200.SparseGSO([(r, c, np.abs(v)) for (r, c, v) in g64.csr], g64.N)
+    twin = gnn_b200.SparseEdgeVariantGF(layer.G, layer.F, layer.K, layer.M, layer.N, layer.E, True).to("cuda", torch.float64)
+    twin.addGSO(g64, device="cuda")
+    with torch.no_grad():
+        twin.weightLSI.copy_(f(layer.weightLSI))
+        twin.bias.copy_(f(layer.bias))
+        for p64, p, pe64, pe in zip(twin.weightEV, layer.weightEV, twin._struct.per_e, layer._struct.per_e):
+            assert torch.equal(pe64["col"], pe["col"]) and torch.equal(pe64["rowptr"], pe["rowptr"])
+            p64.copy_(f(p))
+    x64 = f(x).requires_grad_(True)
+    y64 = twin(x64)
+    y64.backward(f(dy))
+    return y64.detach(), x64.grad, [p.grad for p in twin.weightEV]
+
+
 @pytest.mark.gpu
 def test_sparse_edge_variant_cfg4_size():
     """BASELINE.json config 4 at its stated size: N = 200k, E = 4, K = 3, G = F = 32, hybrid with M = 1024 selected nodes —
     the reference layer would need 32*4*3*32*4e10 parameters.  Constructs, runs forward + backward, and checks the EV part
-    against an fp64 evaluation of the same chains on a sub-sample of (f, g) pairs."""
+    against an fp64 evaluation of the same chains on a sub-sample of (f, g) pairs.  y, x.grad and every weightEV[e].grad
+    are held componentwise to the envelope of ev_oracle / lsigf_oracle around the same layer run in fp64 through the same
+    kernels (their fp64 results are pinned by tests/test_kernel_dispatch.py), M taken from an fp64 run on absolute values."""
+    import ev_oracle as evo
     import gnn_b200
     from gnn_b200 import graphs
     N, M, E, K, G, F, B = 200_000, 1024, 4, 3, 32, 32, 8
@@ -210,11 +235,29 @@ def test_sparse_edge_variant_cfg4_size():
     n_par = sum(p.numel() for p in layer.weightEV)
     assert st.NA < N // 4 and 1e7 < n_par < 1e9
     x = torch.randn(B, G, N, device="cuda", requires_grad=True)
+    dy = torch.randn(B, F, N, device="cuda")
     y = layer(x)
-    y.square().mean().backward()
+    y.backward(dy)
     torch.cuda.synchronize()
     assert tuple(y.shape) == (B, F, N) and torch.isfinite(y).all() and torch.isfinite(x.grad).all()
     assert all(torch.isfinite(p.grad).all() for p in layer.weightEV)
+    # componentwise against the fp64 twin.  Depths c: the EV chains' (ev_depths, worst e) and the LSI part's as in
+    # lsigf_envelope (3xTF32 tensor cores in fp32), plus the E + 2 sums that join the parts (EV over e, LSI, two biases)
+    y64, dx64, dw64 = _twin_fp64(layer, gso, x, dy, absolute=False)
+    yM, dxM, dwM = _twin_fp64(layer, gso, x, dy, absolute=True)
+    depths = [evo.ev_depths(pe["rowptr"].cpu().numpy(), pe["col"].cpu().numpy(), K, G, F, B) for pe in st.per_e]
+    nnz_row = max(max(np.diff(rp).max(), np.bincount(c, minlength=N).max()) for (rp, c, _) in gso.csr)
+    hop, T = (K - 1) * int(nnz_row), 1 + E * (K - 1)
+    u, tc = orc.unit_roundoff(np.float32), orc.TF32X3_PER_PRODUCT
+    checks = [("y", y, y64, yM, max(max(d["Y"] for d in depths), hop + T * G + 2) + E + 2),
+              ("x.grad", x.grad, dx64, dxM, max(max(d["dxT"] for d in depths), hop + T * F + 2) + E + 2)]
+    checks += [("weightEV[%d].grad" % e, p.grad, dw64[e], dwM[e], depths[e]["dw"]) for e, p in enumerate(layer.weightEV)]
+    for name, got, ref, mag, c in checks:
+        extra = tc if name in ("y", "x.grad") else 0.0
+        bound = (c * u + extra) * mag + 4.0 * np.finfo(np.float32).tiny * (c + 1)
+        v = float(((got.double() - ref).abs() / bound).max())
+        print("cfg4 %s: worst error / bound %.3g" % (name, v))
+        assert v <= 1.0, (name, v)
     # EV part alone (sparse fp64 chains for two (f, g) pairs, every e): Y_ev = layer(x) - LSI part - 2 bias
     with torch.no_grad():
         lsi = gnn_b200.LSIGF(layer.weightLSI, gso, x, layer.bias) + layer.bias

@@ -2,8 +2,9 @@
 
 Every row of CASES names an entry point, the shape / layout / alignment that selects a branch, and the kernels that
 branch must launch (regexes on the demangled name, template arguments included).  The GPU test runs the case once under
-torch.profiler, asserts those kernels ran, then checks every output against oracle/lsigf_oracle.py's componentwise bound,
-checks that memory outside the kernel's contract kept its canary pattern, and that a second run is bit-identical.
+torch.profiler, asserts those kernels ran, then checks every output against oracle/lsigf_oracle.py's componentwise bound
+(oracle/ev_oracle.py's for the edge-variant filter), checks that memory outside the kernel's contract kept its canary
+pattern, and that a second run is bit-identical.
 The CPU tests keep the table honest: every __global__ function in csrc/ is covered by a case or excluded with a reason,
 and every regex matches a kernel instantiated in the built library.
 
@@ -22,6 +23,7 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+import ev_oracle as evo
 import lsigf_oracle as orc
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -662,20 +664,146 @@ def _layer_rows():
     return rows
 
 
-CASES = _hop_rows() + _contract_rows() + _tap_grad_rows() + _bias_grad_rows() + _lsigf_rows() + _layout_rows() + _layer_rows()
+# ------------------------------------------------------------------------------------------------ edge-variant filter
+def _ev_pattern(graph, N, diag):
+    """The edge-variant structure (gnn_b200.edgevariant.EVStructure, so the transposed pattern and perm come from the
+    product code) of _graph(graph, N)'s pattern.  diag adds the diagonal on every row i % 4 != 1: the other rows have
+    diag[i] = -1 unless the graph has a self-loop there."""
+    from gnn_b200 import edgevariant as evm
+    m = _graph(graph, N)
+    pat = sp.csr_matrix((np.ones(m.nnz), m.indices, m.indptr), shape=m.shape)
+    if diag:
+        d = np.nonzero(np.arange(N) % 4 != 1)[0]
+        pat = sp.csr_matrix(pat + sp.csr_matrix((np.ones(len(d)), (d, d)), shape=(N, N)))
+    pat.sum_duplicates()
+    pat.sort_indices()
+    rows = np.repeat(np.arange(N), np.diff(pat.indptr))
+    st = evm.EVStructure.from_coo(N, [(torch.from_numpy(rows), torch.from_numpy(pat.indices.astype(np.int64)))], "cuda")
+    return st.per_e[0], st.NA
+
+
+def _ev_case(dtype, B, G, K, F=3, diag=True, N=3000, graph="rand", misaligned=False, pingpong=False):
+    """b200gf_ev_forward + b200gf_ev_backward through the C ABI against oracle/ev_oracle.py.  Y, states, lam, dw and dxT
+    start as NaN and are followed by 4 KB of SENT; the k = 0 weights are non-zero on every slot, so a diag step that read
+    the whole row would show.  misaligned: Y and dY one element past a 16-byte boundary, which selects the VB = 1
+    kernels; their per-element operation order is the vector kernels', so Y, dw and dxT must equal the aligned run bit
+    for bit.  pingpong: a forward with n_states = 2 (inference) must give the Y of n_states = K - 1."""
+    memo = {}
+
+    def run():
+        cabi, lib = _lib()
+        enum = cabi.F32 if dtype == F32 else cabi.F64
+        if not memo:
+            pe, NA = _ev_pattern(graph, N, diag)
+            rng = np.random.default_rng(NA + 7 * B + 31 * G + K)
+            r = lambda shape: orc.biased_uniform(rng, shape).astype(NPD[dtype]).astype(np.float64)   # noqa: E731
+            w, xT, dY = r((F, K, G, pe["nnz"])), r((G, NA, B)), r((F, NA, B))
+            host = [pe[k].cpu().numpy() for k in ("rowptr", "col")] + [pe["diag"].cpu().numpy() if diag else None]
+            Yr, _ = evo.ev_forward(*host, w, xT)
+            dwr, dxr, _ = evo.ev_backward(*host, w, xT, dY)
+            memo.update(pe=pe, NA=NA, w=w, xT=xT, dY=dY, ref=(Yr, dwr, dxr),
+                        env=evo.ev_envelope(*host, w, xT, dY, dtype=NPD[dtype]))
+        pe, NA = memo["pe"], memo["NA"]
+        nnz = pe["nnz"]
+        dev = lambda a: torch.tensor(a, dtype=dtype, device="cuda")          # noqa: E731
+        w, xT = dev(memo["w"]), dev(memo["xT"])
+        pad = 4096 // w.element_size()
+        chain, ny, nw, nx = F * G * NA * B, F * NA * B, F * K * G * nnz, G * NA * B
+        diag_p = pe["diag"].data_ptr() if diag else None
+
+        def buf(n, off=0):
+            t = torch.full((off + n + pad,), SENT, dtype=dtype, device="cuda")
+            t[off:off + n] = float("nan")
+            return t
+
+        def fwd_bwd(n_states, off, backward=True):
+            Yb, Sb = buf(ny, off), buf(n_states * chain)
+            _check(lib.b200gf_ev_forward(enum, NA, B, G, F, K, pe["rowptr"].data_ptr(), pe["col"].data_ptr(), diag_p, nnz,
+                                         w.data_ptr(), xT.data_ptr(), Sb.data_ptr(), n_states, Yb[off:].data_ptr(), _st()))
+            bufs = dict(Y=(Yb, off, ny), states=(Sb, 0, n_states * chain))
+            if backward:
+                dYb = torch.full((off + ny,), float("nan"), dtype=dtype, device="cuda")
+                dYb[off:] = dev(memo["dY"]).flatten()
+                lam, dw, dx = buf(2 * chain), buf(nw), buf(nx)
+                _check(lib.b200gf_ev_backward(enum, NA, B, G, F, K, pe["rowptr"].data_ptr(), pe["col"].data_ptr(),
+                                              pe["rowptrT"].data_ptr(), pe["colT"].data_ptr(), pe["perm"].data_ptr(), diag_p,
+                                              nnz, w.data_ptr(), xT.data_ptr(), Sb.data_ptr(), dYb[off:].data_ptr(),
+                                              lam.data_ptr(), dw.data_ptr(), dx.data_ptr(), _st()))
+                bufs.update(lam=(lam, 0, 2 * chain), dw=(dw, 0, nw), dxT=(dx, 0, nx))
+            return bufs
+
+        res = Result()
+
+        def fence(bufs, tag=""):
+            for name, (t, off, n) in bufs.items():
+                res.canaries += [(tag + name + " before", t[:off]), (tag + name + " tail", t[off + n:])]
+            return bufs
+
+        bufs = fence(fwd_bwd(max(K - 1, 1), 1 if misaligned else 0))
+        Y =bufs["Y"][0][bufs["Y"][1]:][:ny].view(F, NA, B)
+        dw = bufs["dw"][0][:nw].view(F, K, G, nnz)
+        dx = bufs["dxT"][0][:nx].view(G, NA, B)
+        env = memo["env"]
+        res.checks += [(n, t, ref, env[n]) for n, t, ref in zip(("Y", "dw", "dxT"), (Y, dw, dx), memo["ref"])]
+        res.finite += [("Y", Y), ("dw (every slot written)", dw), ("dxT", dx)]
+        res.outputs += [Y, dw, dx]
+        if diag:                                 # the k = 0 off-diagonal slots are written, with exactly 0
+            off_diag = torch.ones(nnz, dtype=torch.bool, device="cuda")
+            d = pe["diag"]
+            off_diag[d[d >= 0].long()] = False
+            assert bool((dw[:, 0][..., off_diag] == 0).all()), "k = 0 off-diagonal dw slots must be exactly 0"
+        if misaligned:
+            al = fence(fwd_bwd(max(K - 1, 1), 0), "aligned ")
+            for n, t in (("Y", Y), ("dw", dw), ("dxT", dx)):
+                assert torch.equal(_bits(t.flatten()), _bits(al[n][0][:t.numel()])), "%s: VB = 1 and VB = 4 differ" % n
+        if pingpong:
+            pp = fence(fwd_bwd(2, 0, backward=False), "ping-pong ")
+            assert torch.equal(_bits(Y.flatten()), _bits(pp["Y"][0][:ny])), "n_states = 2 and n_states = K-1 differ"
+        return res
+    return run
+
+
+def _ev_rows():
+    fwd_bwd = lambda t, vb: [r"step_kernel<%s,%d,8>" % (t, vb), r"adjoint_step_kernel<%s,%d>" % (t, vb),   # noqa: E731
+                             r"adjoint_init_kernel<%s>" % t, r"wgrad_kernel<%s>" % t, r"xgrad_kernel<%s>" % t]
+    rows = [
+        # 16-byte batch vectors, the G-tail of the GB = 8 loop (G = 9), diag with k = 0 off-diagonal weights
+        ("ev-f32-B8-G9-K3-diag", _ev_case(F32, 8, 9, 3), fwd_bwd("float", 4)),
+        ("ev-f32-B7-G17-K3", _ev_case(F32, 7, 17, 3, diag=False), fwd_bwd("float", 1)),
+        # Y / dY misaligned: the VB = 1 kernels, bit-identical to the aligned (VB = 4) run made in the same case
+        ("ev-f32-B8-G8-K2-misaligned", _ev_case(F32, 8, 8, 2, diag=False, misaligned=True),
+         fwd_bwd("float", 1) + [r"step_kernel<float,4,8>", r"adjoint_step_kernel<float,4>"]),
+        # B > 32: wgrad's lane loop
+        ("ev-f64-B33-G1-K4-diag", _ev_case(F64, 33, 1, 4), fwd_bwd("double", 1)),
+        # K = 1: no adjoint step, xgrad on the diag branch
+        ("ev-f64-B64-G20-K1-diag", _ev_case(F64, 64, 20, 1),
+         [r"step_kernel<double,1,8>", r"adjoint_init_kernel<double>", r"wgrad_kernel<double>", r"xgrad_kernel<double>"]),
+        ("ev-f32-B16-G4-K5-diag-pingpong", _ev_case(F32, 16, 4, 5, pingpong=True), fwd_bwd("float", 4)),
+        # the 20 000-entry hub row and column, F NA B / VB > 132 * 16 * 256: every grid-stride loop takes several passes
+        ("ev-hub-f32", _ev_case(F32, 16, 2, 3, F=8, diag=False, N=24000), fwd_bwd("float", 4)),
+        ("ev-hub-f64", _ev_case(F64, 16, 2, 3, F=8, diag=False, N=24000), fwd_bwd("double", 1)),
+    ]
+    for N in (1, 3, 7):
+        rows.append(("ev-tinyN%d-f64" % N, _ev_case(F64, 1, 1, 2, N=N, graph="tiny"), fwd_bwd("double", 1)))
+    return rows
+
+
+CASES = (_hop_rows() + _contract_rows() + _tap_grad_rows() + _bias_grad_rows() + _lsigf_rows() + _layout_rows()
+         + _layer_rows() + _ev_rows())
 
 # __global__ functions without a case here, and where they are tested
+EGATE = "edge-gated layer: tests/test_edge_gated.py keeps its own case table with a GPU case per egate.cu kernel"
 EXCLUDED = {
     "peer_signal_kernel": "multi-process peer fence: tests/test_distributed.py",
     "peer_wait_kernel": "multi-process peer fence: tests/test_distributed.py",
     "bcast_rows_kernel": "all-gather epilogue of the node-sharded path: tests/test_cabi.py, tests/test_distributed.py",
     "scatter_rows_kernel": "scatter epilogue of the feature-sharded path: tests/test_cabi.py, tests/test_distributed.py",
     "narrow_rowptr_kernel": "device plan build (b200gf_plan_create_device): tests/test_widen_*",
-    "step_kernel": "edge-variant filter: tests/test_evgf.py",
-    "adjoint_init_kernel": "edge-variant filter: tests/test_evgf.py",
-    "adjoint_step_kernel": "edge-variant filter: tests/test_evgf.py",
-    "wgrad_kernel": "edge-variant filter: tests/test_evgf.py",
-    "xgrad_kernel": "edge-variant filter: tests/test_evgf.py",
+    "egate_softmax_kernel": EGATE,
+    "egate_softmax_bwd_kernel": EGATE,
+    "egate_colsum_kernel": EGATE,
+    "egate_hop_kernel": EGATE,
+    "egate_sddmm_kernel": EGATE,
 }
 
 
@@ -690,13 +818,15 @@ def _global_functions():
     names = set()
     for path in glob.glob(os.path.join(CSRC, "*.cu")) + glob.glob(os.path.join(CSRC, "*.cuh")):
         src = open(path).read()
-        names.update(re.findall(r"__global__\s+void\s+(?:__launch_bounds__\([^)]*\)\s*)?(\w+)\s*\(", src))
+        # __launch_bounds__ may come before or after the return type
+        names.update(re.findall(r"__global__\s+(?:__launch_bounds__\([^)]*\)\s*)?void\s+(?:__launch_bounds__\([^)]*\)\s*)?"
+                                r"(\w+)\s*\(", src))
     return names
 
 
 def test_every_global_function_has_a_case_or_an_exclusion():
     names = _global_functions()
-    assert len(names) >= 25, sorted(names)
+    assert len(names) >= 36, sorted(names)
     covered = {re.match(r"\w+", k).group(0) for _, _, ks in CASES for k in ks}
     missing = sorted(n for n in names if n not in covered and n not in EXCLUDED)
     assert not missing, "kernels without a dispatch case or an exclusion: %s" % missing
