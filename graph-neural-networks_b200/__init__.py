@@ -12,6 +12,7 @@ from .pooling import MaxPoolLocal  # noqa: F401,E402
 from .activations import MaxLocalActivation, MedianLocalActivation, NoActivation  # noqa: F401,E402
 from .recurrent import GatedGRNN, HiddenState, TimeGatedHiddenState, NodeGatedHiddenState  # noqa: F401,E402
 from .edgegated import EdgeGatedGRNN, EdgeGatedHiddenState, EdgeGatePattern  # noqa: F401,E402
+from .nodevariant import NVGF, NodeVariantGF, TapMap, copy_nodes  # noqa: F401,E402
 from .delayed import LSIGF_DB, GraphFilter_DB, GRNN_DB, HiddenState_DB  # noqa: F401,E402
 from .graphed import graphed, GraphedForward  # noqa: F401,E402
 

@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200gf.so")
 SOURCES = ["plan.cu", "spmm.cu", "taps.cu", "layout.cu", "lsigf.cu", "tc_contract.cu", "ev.cu", "layer.cu", "dmma_contract.cu",
-           "egate.cu"]
+           "egate.cu", "nv/nv.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-O3,-Wall", "--expt-relaxed-constexpr"]
 

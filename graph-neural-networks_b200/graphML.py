@@ -323,16 +323,18 @@ def fuse_layers(model):
 _SAVED = {}
 
 
-def install(gml=None, edge_gating=False):
+def install(gml=None, edge_gating=False, node_variant=False):
     """Point `alegnn.utils.graphML.LSIGF`, `.GraphFilter`, `.EVGF`, `.EdgeVariantGF`, the local pooling / activation
     layers and the static-GSO recurrent layers at this package.  `edge_gating=True` also points
     `.EdgeGatedHiddenState` at the sparse edge-gated layer (edgegated.py); by default it stays the reference's.
+    `node_variant=True` also points `.NVGF` and `.NodeVariantGF` at the sparse node-variant filter (nodevariant.py);
+    by default they stay the reference's.
 
     `GraphFilter.forward` in the reference looks `LSIGF` up as a module global at call time (graphML.py:2137), so
     this also accelerates its hybrid EdgeVariantGF (:2686), jARMA (:592) and GatedGRNN (:1403,:1461) call sites.
     Architectures built AFTER install() get this package's layers (plan cached in addGSO).
     """
-    from . import activations, delayed, edgegated, edgevariant, pooling, recurrent
+    from . import activations, delayed, edgegated, edgevariant, nodevariant, pooling, recurrent
     if gml is None:
         import alegnn.utils.graphML as gml
     if id(gml) not in _SAVED:
@@ -346,6 +348,12 @@ def install(gml=None, edge_gating=False):
         _SAVED[id(gml)][1].setdefault("EdgeGatedHiddenState", getattr(gml, "EdgeGatedHiddenState"))
         # per-non-zero attention gates and the per-sample gated hop (edgegated.py); gml.GatedGRNN stays the reference's
         gml.EdgeGatedHiddenState = edgegated.EdgeGatedHiddenState
+    if node_variant:
+        for name in ("NVGF", "NodeVariantGF"):
+            _SAVED[id(gml)][1].setdefault(name, getattr(gml, name))
+        # per-node tap contraction on the LSIGF hops; copyNodes by a sparse breadth-first search (nodevariant.py)
+        gml.NVGF = nodevariant.NVGF
+        gml.NodeVariantGF = nodevariant.NodeVariantGF
     gml.LSIGF = LSIGF
     gml.GraphFilter = GraphFilter
     gml.EVGF = edgevariant.EVGF

@@ -327,6 +327,39 @@ int b200gf_gated_hop_backward(int dtype, int64_t N, int Bs, int C,
                               void* dsrc, int64_t dsrc_ld, void* dgate, int64_t dgate_sb, int64_t dgate_sp,
                               void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Node-variant graph filter (NVGF, alegnn/utils/graphML.py:293-387; NodeVariantGF :2317-2509), node-major only:
+ *   y[n, b*F + f] = bias + sum_e sum_k sum_g h[f,e,k,g,node_tap[n]] (x_g S_e^k)[n]
+ * Every node n reads the tap block m = node_tap[n] (int32 [N], 0 <= m < M; the layer's copyNodes), so the reference's
+ * [F,E,K,G,N] index_select of the taps is never materialised.
+ *
+ * b200gf_nv_pack_taps: h [F,E,K,G,M] -> W [M][T][G][F], T = 1 + E*(K-1): W[m][0] = sum_e h[:,e,0,:,m]^T (k = 0 is the
+ *   same x for every e), W[m][1 + e*(K-1) + (k-1)] = h[:,e,k,:,m]^T.  Each node's taps are one contiguous block.
+ * b200gf_nv_forward: the E*(K-1) hops of b200gf_forward into the workspace, then one per-node contraction.  x [N, x_ld],
+ *   y [N, y_ld] (ld >= B*G / B*F); bias NULL, [F] (bias_per_node = 0) or [F, N] (bias_per_node = 1).  Writes nothing at
+ *   or past column B*F of y and no row at or past N.
+ * b200gf_nv_backward: dy [N, dy_ld], x = the forward input.
+ *   dx (NULL to skip) [N, dx_ld]: dz_t[n, b*G+g] = sum_f W[m][t][g][f] dy[n, b*F+f] and
+ *     dx = dz_0 + sum_e BWD(dz_{e,1} + BWD(dz_{e,2} + ... BWD(dz_{e,K-1})));  nothing at or past column B*G is written.
+ *   dh [F,E,K,G,M] (never NULL): dh[f,e,k,g,m] = sum over the nodes n of tap m, sum_b (x_g S_e^k)[n,b] dy[n,b,f]
+ *     (k = 0: the merged term, the same value in every e).  Every dh element is written; taps that no node uses get
+ *     exactly 0.  tap_rowptr (int64 [M+1]) / tap_nodes (int32 [N]) list the nodes of every tap in ascending order (the
+ *     inverse of node_tap).  The sum is a deterministic two-pass reduction over fixed-size pieces of each member list,
+ *     so a tap shared by every node (M = 1) is spread over many blocks.
+ *   dbias (NULL to skip): as b200gf_backward.
+ * workspace: b200gf_nv_workspace_bytes(plan, B, G, F, K, M, backward) bytes, 256-byte aligned.  T <= 48.
+ * ---------------------------------------------------------------------------------------------- */
+int b200gf_nv_pack_taps(int dtype, const void* h, void* W, int F, int E, int K, int G, int64_t M, void* stream);
+int b200gf_nv_forward(const b200gf_plan* plan, const void* x, int64_t x_ld, const void* W, const int32_t* node_tap,
+                      int64_t M, const void* bias, int bias_per_node, void* y, int64_t y_ld,
+                      void* workspace, size_t workspace_bytes, int B, int G, int F, int K, void* stream);
+int b200gf_nv_backward(const b200gf_plan* plan, const void* dy, int64_t dy_ld, const void* x, int64_t x_ld,
+                       const void* W, const int32_t* node_tap, int64_t M,
+                       const int64_t* tap_rowptr, const int32_t* tap_nodes,
+                       void* dx, int64_t dx_ld, void* dh, void* dbias, int bias_per_node,
+                       void* workspace, size_t workspace_bytes, int B, int G, int F, int K, void* stream);
+size_t b200gf_nv_workspace_bytes(const b200gf_plan* plan, int B, int G, int F, int K, int64_t M, int backward);
+
 /* layout conversion between the reference's [C, N] (feature-major, C = B*G) and node-major [N, ld] */
 int b200gf_to_node_major(int dtype, const void* src_cn, void* dst_nc, int64_t dst_ld,
                          int64_t N, int C, void* stream);
