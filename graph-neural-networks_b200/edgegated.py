@@ -195,6 +195,19 @@ class _Attention(torch.autograd.Function):
         return ds, dmixer, None
 
 
+def _row_ld(u):
+    """Leading dimension of node-major u [N, Bs, C].  With N = 1 torch may report any row stride (a permuted [B, H, 1]
+    tensor is already "contiguous" with stride 1); only row 0 is read, so Bs*C is as good as any and the entry points
+    require ld >= Bs*C."""
+    return u.stride(0) if u.shape[0] > 1 else u.shape[1] * u.shape[2]
+
+
+def _gate_ptr(gate, u, pat):
+    """The gate's address.  With an empty mask every S entry lies outside it (pos = -1), so the kernels read no gate,
+    but the empty gate tensor has a null address, which the entry points reject: hand them u's instead."""
+    return gate.data_ptr() if pat.nnz > 0 else u.data_ptr()
+
+
 class _GatedHop(torch.autograd.Function):
     """u [N, Bs, C] (node-major) -> (u S~_b) per sample b, S~_b = gate[b] (.) S;  gate [Bs, nnz] of any strides."""
 
@@ -209,8 +222,8 @@ class _GatedHop(torch.autograd.Function):
         t_val, _, _ = pat.values(u.dtype)
         st = torch.cuda.current_stream().cuda_stream
         _cabi.check(lib.b200gf_gated_hop_forward(_ENUM[u.dtype], N, Bs, C, pat.t_rowptr.data_ptr(), pat.t_col.data_ptr(),
-                                                 t_val.data_ptr(), pat.t_pos.data_ptr(), gate.data_ptr(),
-                                                 gate.stride(0), gate.stride(1), u.data_ptr(), u.stride(0),
+                                                 t_val.data_ptr(), pat.t_pos.data_ptr(), _gate_ptr(gate, u, pat),
+                                                 gate.stride(0), gate.stride(1), u.data_ptr(), _row_ld(u),
                                                  out.data_ptr(), Bs * C, st))
         ctx.pat = pat
         ctx.save_for_backward(u, gate)
@@ -225,15 +238,16 @@ class _GatedHop(torch.autograd.Function):
         dout = dout.contiguous()
         du = torch.empty_like(dout) if ctx.needs_input_grad[0] else None
         dg = torch.empty((pat.nnz, Bs), dtype=u.dtype, device=u.device) if ctx.needs_input_grad[1] else None
-        if du is None and dg is None:
-            return None, None, None
+        if du is None and (dg is None or pat.nnz == 0):          # nothing to write (an empty mask has no gate)
+            return None, None if dg is None else dg.t(), None
         _, s_val, m_sval = pat.values(u.dtype)
         st = torch.cuda.current_stream().cuda_stream
         _cabi.check(lib.b200gf_gated_hop_backward(
             _ENUM[u.dtype], N, Bs, C, pat.s_rowptr.data_ptr(), pat.s_col.data_ptr(), s_val.data_ptr(),
-            pat.s_pos.data_ptr(), pat.m_rowptr.data_ptr(), pat.m_col.data_ptr(), m_sval.data_ptr(), gate.data_ptr(),
-            gate.stride(0), gate.stride(1), u.data_ptr(), u.stride(0), dout.data_ptr(), Bs * C,
-            None if du is None else du.data_ptr(), Bs * C, None if dg is None else dg.data_ptr(), 1, Bs, st))
+            pat.s_pos.data_ptr(), pat.m_rowptr.data_ptr(), pat.m_col.data_ptr(), m_sval.data_ptr(),
+            _gate_ptr(gate, u, pat), gate.stride(0), gate.stride(1), u.data_ptr(), _row_ld(u), dout.data_ptr(), Bs * C,
+            None if du is None else du.data_ptr(), Bs * C, None if dg is None or pat.nnz == 0 else dg.data_ptr(), 1, Bs,
+            st))
         return du, None if dg is None else dg.t(), None
 
 

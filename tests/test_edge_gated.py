@@ -4,12 +4,10 @@ alegnn/utils/graphML.py:4033-4209, GatedGRNN's edge path :1410-1451 / :1474-1514
 
 CPU tests check the host logic (pattern, gate layouts, recursion, autograd wiring) with torch restatements standing in
 for the two kernels (`_attention`, `_gated_hop`) and the dense CPU oracle for the gate GRNNs' filter; GPU tests run
-the real kernels against the fixtures, against the fp64 restatement in oracle/egate_oracle.py, and at scale.
-
-egate.cu's kernels are tested here rather than in the dispatch table of test_kernel_dispatch.py:
-`test_every_egate_kernel_has_a_gpu_case` requires a GPU case below for each of them."""
+the real kernels against the fixtures, against the fp64 restatement in oracle/egate_oracle.py, at scale, and on one-,
+two- and three-node graphs.  Each launch branch of egate.cu's kernels has a componentwise-bounded row in
+tests/test_egate_dispatch.py."""
 import os
-import re
 
 import numpy as np
 import pytest
@@ -18,7 +16,6 @@ import torch
 import egate_oracle as ego
 import lsigf_oracle as orc
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = np.load(os.path.join(os.path.dirname(__file__), "golden", "grnn_edge_cases.npz"))
 TAGS = ["base", "nobias", "k1", "kgt", "relu", "diag", "neg"]
 SIGMA = {0: torch.tanh, 1: torch.relu}
@@ -279,28 +276,7 @@ def test_gated_grnn_points_edge_gates_to_the_new_entry_point():
                       torch.ones(B, T, 1, N), torch.ones(B, H, N), torch.tanh, q, q)
 
 
-def _egate_kernels():
-    src = open(os.path.join(ROOT, "graph-neural-networks_b200", "csrc", "egate.cu")).read()
-    return set(re.findall(r"__global__\s+(?:__launch_bounds__\([^)]*\)\s*)?void\s+(?:__launch_bounds__\([^)]*\)\s*)?(\w+)\s*\(",
-                          src))
-
-
-def test_every_egate_kernel_has_a_gpu_case():
-    names = _egate_kernels()
-    assert names == set(KERNEL_CASES), (sorted(names), sorted(KERNEL_CASES))
-
-
 # ------------------------------------------------------------------------------------------------------------ GPU
-# every kernel of egate.cu and the GPU test that runs it (checked on the CPU above)
-KERNEL_CASES = {
-    "egate_softmax_kernel": "test_attention_kernels_vs_fp64_restatement",
-    "egate_softmax_bwd_kernel": "test_attention_kernels_vs_fp64_restatement",
-    "egate_colsum_kernel": "test_attention_kernels_vs_fp64_restatement",
-    "egate_hop_kernel": "test_gated_hop_kernels_vs_fp64_restatement",
-    "egate_sddmm_kernel": "test_gated_hop_kernels_vs_fp64_restatement",
-}
-
-
 def _random_graph(rng, N, neg_diag=True):
     """Varied degrees: empty rows, degree-1 rows, a hub row and a hub column, S_ii = -1 nodes, explicit diagonals."""
     deg = rng.integers(0, 9, N)
@@ -476,3 +452,49 @@ def test_backward_is_bitwise_reproducible_and_graphed_forward_is_bit_identical()
         fn = gnn_b200.graphed(lambda a, b: layer(a, b)[0], xt, zt)
         replay = fn(xt, zt).clone()
     assert torch.equal(eager, replay)
+
+
+# one-, two- and three-node graphs: S = [[-1]] has an empty mask (every gate is empty, every S entry is gated off)
+TINY_S = {
+    "N1": [[0.5]],
+    "N1-empty-mask": [[-1.0]],
+    "N2": [[0.0, 0.5], [-0.25, 0.0]],
+    "N3": [[0.3, 0.0, -0.5], [0.0, -1.0, 0.25], [0.75, 0.0, 0.0]],
+}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("tag", list(TINY_S))
+def test_tiny_graph_layer_vs_fp64_oracle(tag):
+    """K = 3, B = 2, H = 3 in fp64 against egate_oracle.edge_gated_hidden_state_coo: z, zT and the gradients of x, z0
+    and every parameter.  With N = 1 a node-major hidden state reports a row stride of 1, below Bs*C."""
+    import gnn_b200
+    S = np.array(TINY_S[tag])
+    N = S.shape[0]
+    B, T, F, H, K = 2, 3, 2, 3, 3
+    torch.manual_seed(N)
+    layer = gnn_b200.EdgeGatedHiddenState(F, H, K)
+    layer.addGSO(torch.tensor(S, device="cuda").reshape(1, N, N))
+    layer = layer.double().cuda()
+    rng = np.random.default_rng(N)
+    x, z0, dz = rng.standard_normal((B, T, F, N)), rng.standard_normal((B, H, N)), rng.standard_normal((B, T, H, N))
+    xt = torch.tensor(x, device="cuda", requires_grad=True)
+    zt = torch.tensor(z0, device="cuda", requires_grad=True)
+    z, zT = layer(xt, zt)
+    z.backward(torch.tensor(dz, device="cuda"))
+    p = {k: v.detach().cpu().requires_grad_(True) for k, v in layer.state_dict().items()}
+    x64, z64 = torch.tensor(x, requires_grad=True), torch.tensor(z0, requires_grad=True)
+    rows, cols = np.nonzero(S)
+    zr, _, _, _ = ego.edge_gated_hidden_state_coo(p, N, rows, cols, S[rows, cols], x64, z64, torch.tanh)
+    zr.backward(torch.tensor(dz))
+    assert _rel(z.detach().cpu().numpy(), zr.detach().numpy()) < 1e-10
+    assert _rel(zT.detach().cpu().numpy()[:, 0, 0], zr.detach().numpy()[:, -1]) < 1e-10
+    assert _rel(xt.grad.cpu().numpy(), x64.grad.numpy()) < 1e-10
+    assert _rel(zt.grad.cpu().numpy(), z64.grad.numpy()) < 1e-10
+    for name, prm in layer.named_parameters():
+        ref = np.zeros(tuple(prm.shape)) if p[name].grad is None else p[name].grad.numpy()
+        got = np.zeros(tuple(prm.shape)) if prm.grad is None else prm.grad.cpu().numpy()
+        if not np.any(ref):                                   # an empty mask: the gates reach nothing
+            assert np.abs(got).max(initial=0) < 1e-12, name
+        else:
+            assert _rel(got, ref) < 1e-10, name

@@ -792,7 +792,7 @@ CASES = (_hop_rows() + _contract_rows() + _tap_grad_rows() + _bias_grad_rows() +
          + _layer_rows() + _ev_rows())
 
 # __global__ functions without a case here, and where they are tested
-EGATE = "edge-gated layer: tests/test_edge_gated.py keeps its own case table with a GPU case per egate.cu kernel"
+EGATE = "edge-gated layer: tests/test_egate_dispatch.py keeps its own case table, one row per egate.cu launch branch"
 EXCLUDED = {
     "peer_signal_kernel": "multi-process peer fence: tests/test_distributed.py",
     "peer_wait_kernel": "multi-process peer fence: tests/test_distributed.py",
