@@ -37,6 +37,9 @@ struct CsrDev {
   void* val = nullptr;        // [nnz] of dtype
   int64_t nnz = 0;
   bool owned = true;          // false when it aliases the other direction (symmetric GSO)
+  // most non-zeros lie far from the diagonal, so a hop's gathers spread over the whole source (hop_chunk_lanes);
+  // set by b200gf_plan_create, which sees the host CSR
+  bool spread = false;
 };
 
 inline size_t dtype_size(int dtype) { return dtype == B200GF_F64 ? 8 : 4; }
@@ -65,8 +68,9 @@ struct BcastHost {
 };
 
 // internal launchers (defined across the .cu files) -------------------------------------------------
-int launch_hop(int dtype, int sm_count, const CsrDev& A, int64_t n_rows, const void* src, int64_t src_ld,
-               void* dst, int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh = nullptr,
+// l2_bytes: L2 size the plain hop's column chunks are sized against (hop_chunk_lanes), 0 = row width alone decides
+int launch_hop(int dtype, int sm_count, int64_t l2_bytes, const CsrDev& A, int64_t n_rows, const void* src,
+               int64_t src_ld, void* dst, int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh = nullptr,
                const BcastHost* bh = nullptr);
 int launch_scatter_rows(int dtype, const void* src, int64_t src_ld, int64_t n_rows, int C, cudaStream_t st,
                         const ScatterHost* sh);
@@ -125,6 +129,7 @@ struct b200gf_plan {
   int64_t n_rows = 0, n_cols = 0;
   int E = 0;
   int sm_count = 132;
+  int64_t l2_bytes = 0;   // device L2 size the hops size their column chunks against (b200gf_plan_set_l2_bytes)
   bool symmetric = false;
   bool has_bwd = false;
   std::vector<b200gf::CsrDev> fwd;  // CSR of S_e^T rows: forward shift gather operator

@@ -89,7 +89,9 @@ int plan_hop(const b200gf_plan* p, const CsrDev& A, const void* src, int64_t src
              cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
   const bool prof = p->prof_used < (int)p->prof_start.size();
   if (prof) CUDA_TRY(cudaEventRecord(p->prof_start[p->prof_used], st));
-  const int rc = launch_hop(p->dtype, p->sm_count, A, p->n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
+  // partitioned plans (one node shard per GPU) keep the chunk width of their row width
+  const int64_t l2 = p->n_rows == p->n_cols ? p->l2_bytes : 0;
+  const int rc = launch_hop(p->dtype, p->sm_count, l2, A, p->n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
   if (prof) {
     CUDA_TRY(cudaEventRecord(p->prof_stop[p->prof_used], st));
     p->prof_used++;

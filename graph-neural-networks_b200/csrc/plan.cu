@@ -1,5 +1,6 @@
 // Plan = device-resident CSR gather operators for the GSO.  Replaces GraphFilter.addGSO's dense E x N x N
 // tensor (reference alegnn/utils/graphML.py:2116-2123).
+#include <cstdlib>
 #include <cstring>
 #include <new>
 #include <string>
@@ -114,6 +115,9 @@ int init_device(b200gf_plan* p, int device) {
   CUDA_TRY(cudaSetDevice(device));
   p->device = device;
   p->sm_count = prop.multiProcessorCount;
+  int l2 = 0;
+  CUDA_TRY(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, device));
+  p->l2_bytes = l2;
   return B200GF_OK;
 }
 
@@ -196,12 +200,20 @@ int b200gf_plan_create(b200gf_plan** out, int device, int64_t N, int E, const in
     if ((rc = validate_csr(A, N, N))) break;
     if ((rc = transpose_host(A, N, es, At))) break;
     const bool sym = A.rowptr == At.rowptr && A.col == At.col && A.val == At.val;
+    // |i - j| > N/8 holds for 77 % of the non-zeros of a graph without locality (Erdos-Renyi), and for few of a graph
+    // numbered community by community
+    int64_t far = 0;
+    for (int64_t i = 0; i < N; ++i)
+      for (int64_t j = A.rowptr[i]; j < A.rowptr[i + 1]; ++j) far += 8 * std::abs(i - (int64_t)A.col[j]) > N;
+    const bool spread = 2 * far > A.rowptr[N];
     all_sym = all_sym && sym;
     if ((rc = upload(At, N, es, p->fwd[e]))) break;   // forward gathers along columns of S_e
+    p->fwd[e].spread = spread;
     if (sym) {
       p->bwd[e] = p->fwd[e];
       p->bwd[e].owned = false;
     } else if ((rc = upload(A, N, es, p->bwd[e]))) break;
+    p->bwd[e].spread = spread;
   }
   if (rc) { b200gf_plan_destroy(p); return rc; }
   p->symmetric = all_sym;
@@ -317,8 +329,15 @@ int64_t b200gf_plan_info(const b200gf_plan* plan, int what) {
     case 4: return plan->device;
     case 5: { int64_t s = 0; for (auto& d : plan->fwd) s += d.nnz; return s; }
     case 6: return plan->symmetric ? 1 : 0;
+    case 7: return plan->l2_bytes;
     default: return B200GF_EINVAL;
   }
+}
+
+int b200gf_plan_set_l2_bytes(b200gf_plan* plan, int64_t bytes) {
+  if (!plan || bytes < 0) return B200GF_EINVAL;
+  plan->l2_bytes = bytes;
+  return B200GF_OK;
 }
 
 }  // extern "C"

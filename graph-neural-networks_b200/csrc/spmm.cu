@@ -99,7 +99,9 @@ template <typename T, int L, int SCATTER>
 static int launch_v2(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst, int64_t dst_ld,
                      int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
   constexpr int VEC = 32 / sizeof(T), U = 4, THREADS = 256, MINB = sizeof(T) == 4 ? 4 : 3, HINT = B200GF_HOP_L2_HINT;
-  auto kern = spmm_hop_v2_kernel<T, int32_t, VEC, L, U, THREADS, MINB, HINT, SCATTER>;
+  // streaming stores (SH = 1): the result rows are read by the next launch, not by this one, so at normal priority they
+  // only displace gathered lines from the L2 (2.74 against 2.78 ms per hop at N = 1M, 64 fp32 columns)
+  auto kern = spmm_hop_v2_kernel<T, int32_t, VEC, L, U, THREADS, MINB, HINT, SCATTER, 1>;
   if (n_rows == 0) return B200GF_OK;
   const int n_chunks = (C + L * VEC - 1) / (L * VEC);
   if (n_chunks > 65535) return B200GF_EUNSUPPORTED;
@@ -156,8 +158,32 @@ static int launch_multirow_v2(int sm_count, const CsrDev& A, int64_t n_rows, con
   return B200GF_OK;
 }
 
+// Lane count L (chunk = L x 32 bytes of each row) of spmm_hop_v2_kernel for rows of nw 32-byte vectors.  The kernel runs
+// the chunks chunk-major, so what the resident warps gather from at any time is one chunk of every source row, n_src * L
+// * 32 bytes.  By default the row width alone sets L (at most 32 lanes, 1 KB chunks).  When that chunk does not fit the
+// L2, the widest narrower chunk (L = 16, 8 or 4) that fits is used: every extra chunk re-reads col/val once, far fewer
+// bytes than gathering rows that miss the L2 from HBM.  L >= 4 keeps a chunk whole 128-byte L2 lines.  When not even
+// L = 4 fits, the default stays.
+// The budget is the whole L2: on an H100 (50 MB L2) chunks of 51.2 MB ran as fast as chunks of 25.6 MB (N = 100k,
+// 2048 fp32 columns) or faster (N = 200k, 1024 fp32 columns: 3.51 against 3.58 ms per hop), while 102 MB chunks were
+// 11 % slower.
+// When not even L = 4 fits, two 128-byte chunks of a 256-byte row still raise the share of gathers that hit the L2 if
+// the gathers spread over the whole source (`spread`) and a chunk is at most 3x the L2: 2.69 against 2.74 ms per hop
+// at N = 1M with 64 fp32 columns (128 MB chunks).  They cost time at 5x the L2 (N = 2M: 6.16 against 5.92 ms), on a
+// graph numbered community by community, whose gathers stay near the diagonal (2.19 against 2.17 ms), and as four
+// chunks of a 512-byte row (64 fp64 columns: 5.80 against 5.70 ms), which read col/val four times.
+static int hop_chunk_lanes(int64_t n_src, int nw, int64_t l2_bytes, bool spread) {
+  const int L0 = nw <= 8 ? 8 : nw <= 16 ? 16 : 32;
+  const auto fits = [&](int L) { return n_src * 32 * (L < nw ? L : nw) <= l2_bytes; };
+  if (fits(L0)) return L0;
+  for (int L = L0 / 2; L >= 4; L /= 2)
+    if (fits(L)) return L;
+  if (spread && nw > 4 && nw <= 8 && n_src * 32 * 4 <= 3 * l2_bytes) return 4;
+  return L0;
+}
+
 template <typename T>
-static int launch_typed(int sm_count, const CsrDev& A, int64_t n_rows, const void* src_, int64_t src_ld,
+static int launch_typed(int sm_count, int64_t l2_bytes, const CsrDev& A, int64_t n_rows, const void* src_, int64_t src_ld,
                         void* dst_, int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
   constexpr int VEC = 16 / sizeof(T);
   const T* src = reinterpret_cast<const T*>(src_);
@@ -225,22 +251,25 @@ static int launch_typed(int sm_count, const CsrDev& A, int64_t n_rows, const voi
     wide_ok = wide_ok && sh->gl % VW == 0 && sh->out_ld % VW == 0 && sh->out_col % VW == 0 && sh->stride_b % VW == 0;
   if (wide_ok) {
     const int nw = Cw / VW;  // 32-byte vectors per row
-    if (nw <= 8) return launch_v2_sc<T, 8>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
-    if (nw <= 16) return launch_v2_sc<T, 16>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
+    // the feature-sharded scatter keeps the chunk width of its row width
+    const int L = hop_chunk_lanes(n_rows, nw, sh && sh->n_peers > 0 ? 0 : l2_bytes, A.spread);
+    if (L == 4) return launch_v2_sc<T, 4>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
+    if (L == 8) return launch_v2_sc<T, 8>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
+    if (L == 16) return launch_v2_sc<T, 16>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
     return launch_v2_sc<T, 32>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
   }
   if (nv <= 16) return launch_one<T, VEC, 16, 4>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
   return launch_one<T, VEC, 32, 4>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
 }
 
-int launch_hop(int dtype, int sm_count, const CsrDev& A, int64_t n_rows, const void* src, int64_t src_ld,
-               void* dst, int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
+int launch_hop(int dtype, int sm_count, int64_t l2_bytes, const CsrDev& A, int64_t n_rows, const void* src,
+               int64_t src_ld, void* dst, int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
   if (C <= 0 || src_ld < C || (!bh && dst_ld < C)) return B200GF_EINVAL;
   if (sh && (sh->n_peers < 0 || sh->n_peers > MAX_PEERS)) return B200GF_EINVAL;
   if (bh && (bh->n_peers < 0 || bh->n_peers > MAX_PEERS || (bh->n_peers > 0 && bh->out_ld < C))) return B200GF_EINVAL;
   if (bh && bh->n_peers == 0 && !(sh && sh->n_peers > 0)) return B200GF_EINVAL;   // no all-gather only in the grid epilogue
-  if (dtype == B200GF_F32) return launch_typed<float>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
-  if (dtype == B200GF_F64) return launch_typed<double>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
+  if (dtype == B200GF_F32) return launch_typed<float>(sm_count, l2_bytes, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
+  if (dtype == B200GF_F64) return launch_typed<double>(sm_count, l2_bytes, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
   return B200GF_EUNSUPPORTED;
 }
 

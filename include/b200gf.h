@@ -96,8 +96,14 @@ int b200gf_plan_create_device(b200gf_plan** out, int device, int64_t N, int E,
 void b200gf_plan_destroy(b200gf_plan* plan);
 
 /* introspection: what = 0 n_rows, 1 n_cols, 2 E, 3 dtype, 4 device, 5 nnz (sum over e, forward operator),
- * 6 symmetric (1 if every S_e == S_e^T bit-for-bit, so both operators share storage) */
+ * 6 symmetric (1 if every S_e == S_e^T bit-for-bit, so both operators share storage), 7 L2 bytes the hops size their
+ * column chunks against (b200gf_plan_set_l2_bytes) */
 int64_t b200gf_plan_info(const b200gf_plan* plan, int what);
+
+/* L2 size (bytes) the plan's hops size their gathered column chunks against; plan creation reads it from the device
+ * (cudaDevAttrL2CacheSize).  0 turns the sizing off: every hop then uses the chunk width its row width alone selects.
+ * Results differ only by the summation order of the chunk fold.  For A/B timing and tests; bytes < 0 is EINVAL. */
+int b200gf_plan_set_l2_bytes(b200gf_plan* plan, int64_t bytes);
 
 /* ------------------------------------------------------------------------------------------------
  * LSIGF forward  (graphML.py:83-176)
