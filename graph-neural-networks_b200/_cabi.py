@@ -75,6 +75,11 @@ _SIGNATURES = {
     "b200gf_nv_backward": (c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,
                                    c_int, c_vp, c_sz, c_int, c_int, c_int, c_int, c_vp]),
     "b200gf_nv_workspace_bytes": (c_sz, [c_vp, c_int, c_int, c_int, c_int, c_i64, c_int]),
+    "b200gf_arma_forward": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_i64, c_vp, c_i64,
+                                    c_vp, c_vp, c_sz, c_vp]),
+    "b200gf_arma_backward": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_i64, c_vp, c_vp,
+                                     c_i64, c_vp, c_vp, c_vp, c_sz, c_vp]),
+    "b200gf_arma_workspace_bytes": (c_sz, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int]),
     "b200gf_tap_contract":(c_int, [c_int, c_i64, c_int, c_int, c_int, c_int, PP, ctypes.POINTER(c_i64), c_vp, c_vp,
                                     c_int, c_vp, c_i64, c_int, c_vp, c_sz, c_vp]),
     "b200gf_tap_contract_scratch_bytes": (c_sz, [c_int, c_int, c_int]),

@@ -12,7 +12,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200gf.so")
 SOURCES = ["plan.cu", "spmm.cu", "taps.cu", "layout.cu", "lsigf.cu", "tc_contract.cu", "ev.cu", "layer.cu", "dmma_contract.cu",
-           "egate.cu", "nv/nv.cu"]
+           "egate.cu", "nv/nv.cu",
+           # beside csrc/, not under it: see the header of csrc_arma/arma.cu
+           "../csrc_arma/arma.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-O3,-Wall", "--expt-relaxed-constexpr"]
 

@@ -187,23 +187,30 @@ def LSIGF(h, S, x, b=None, activation=None):
     B = x.shape[0]
     assert x.shape[1] == G                       # graphML.py:139
     assert x.shape[2] == N                       # graphML.py:140
-    if b is not None:
-        # the reference adds b by broadcasting (graphML.py:174-175): GraphFilter passes [F, 1], and the reference's own
-        # GatedGRNN reshapes its biases to (1, F, 1) before calling LSIGF (graphML.py:1394-1404, :1461)
-        if b.dim() == 3 and b.shape[0] == 1:
-            b = b[0]
-        elif b.dim() == 1 and N == 1:
-            b = b.reshape(-1, 1)
-        if not (b.dim() == 2 and b.shape[0] in (1, F_) and b.shape[1] in (1, N)):
-            raise RuntimeError("b200gf: LSIGF bias must broadcast against [B, F, N] as [F, 1], [F, N], [1, F, 1] or "
-                               "[1, F, N]; got %s" % (tuple(b.shape),))
-        if b.shape[0] == 1 and F_ > 1:
-            b = b.expand(F_, b.shape[1])
+    b = _bias_2d(b, F_, N, "LSIGF")
     if activation is None:
         return _dispatch(h, S, x, b)
     if activation != "relu":
         raise ValueError("b200gf: fused activation must be None or 'relu', got %r" % (activation,))
     return _dispatch(h, S, x, b, 1)
+
+
+def _bias_2d(b, F_, N, name):
+    """The bias forms LSIGF accepts, as [F, 1] or [F, N] (None stays None)."""
+    if b is None:
+        return None
+    # the reference adds b by broadcasting (graphML.py:174-175): GraphFilter passes [F, 1], and the reference's own
+    # GatedGRNN reshapes its biases to (1, F, 1) before calling LSIGF (graphML.py:1394-1404, :1461)
+    if b.dim() == 3 and b.shape[0] == 1:
+        b = b[0]
+    elif b.dim() == 1 and N == 1:
+        b = b.reshape(-1, 1)
+    if not (b.dim() == 2 and b.shape[0] in (1, F_) and b.shape[1] in (1, N)):
+        raise RuntimeError("b200gf: %s bias must broadcast against [B, F, N] as [F, 1], [F, N], [1, F, 1] or "
+                           "[1, F, N]; got %s" % (name, tuple(b.shape)))
+    if b.shape[0] == 1 and F_ > 1:
+        b = b.expand(F_, b.shape[1])
+    return b
 
 
 def _dispatch_cuda(h, S, x, b, act=0):
@@ -323,18 +330,19 @@ def fuse_layers(model):
 _SAVED = {}
 
 
-def install(gml=None, edge_gating=False, node_variant=False):
+def install(gml=None, edge_gating=False, node_variant=False, arma=False):
     """Point `alegnn.utils.graphML.LSIGF`, `.GraphFilter`, `.EVGF`, `.EdgeVariantGF`, the local pooling / activation
     layers and the static-GSO recurrent layers at this package.  `edge_gating=True` also points
     `.EdgeGatedHiddenState` at the sparse edge-gated layer (edgegated.py); by default it stays the reference's.
     `node_variant=True` also points `.NVGF` and `.NodeVariantGF` at the sparse node-variant filter (nodevariant.py);
-    by default they stay the reference's.
+    by default they stay the reference's.  `arma=True` also points `.jARMA` and `.GraphFilterARMA` at the sparse ARMA
+    filter (arma.py); by default they stay the reference's (whose residue term still runs on this package's LSIGF).
 
     `GraphFilter.forward` in the reference looks `LSIGF` up as a module global at call time (graphML.py:2137), so
     this also accelerates its hybrid EdgeVariantGF (:2686), jARMA (:592) and GatedGRNN (:1403,:1461) call sites.
     Architectures built AFTER install() get this package's layers (plan cached in addGSO).
     """
-    from . import activations, delayed, edgegated, edgevariant, nodevariant, pooling, recurrent
+    from . import activations, arma as arma_mod, delayed, edgegated, edgevariant, nodevariant, pooling, recurrent
     if gml is None:
         import alegnn.utils.graphML as gml
     if id(gml) not in _SAVED:
@@ -354,6 +362,12 @@ def install(gml=None, edge_gating=False, node_variant=False):
         # per-node tap contraction on the LSIGF hops; copyNodes by a sparse breadth-first search (nodevariant.py)
         gml.NVGF = nodevariant.NVGF
         gml.NodeVariantGF = nodevariant.NodeVariantGF
+    if arma:
+        for name in ("jARMA", "GraphFilterARMA"):
+            _SAVED[id(gml)][1].setdefault(name, getattr(gml, name))
+        # sparse Jacobi chains on the S~ plan instead of [F,E,P,G,N,N] dense operators (arma.py)
+        gml.jARMA = arma_mod.jARMA
+        gml.GraphFilterARMA = arma_mod.GraphFilterARMA
     gml.LSIGF = LSIGF
     gml.GraphFilter = GraphFilter
     gml.EVGF = edgevariant.EVGF

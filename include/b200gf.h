@@ -366,6 +366,39 @@ int b200gf_nv_backward(const b200gf_plan* plan, const void* dy, int64_t dy_ld, c
                        void* workspace, size_t workspace_bytes, int B, int G, int F, int K, void* stream);
 size_t b200gf_nv_workspace_bytes(const b200gf_plan* plan, int B, int G, int F, int K, int64_t M, int backward);
 
+/* ------------------------------------------------------------------------------------------------
+ * ARMA graph filter by Jacobi iterations (jARMA, alegnn/utils/graphML.py:490-638; GraphFilterARMA :2714-2847), the
+ * general-diagonal part (H1 + H2; the residue H3 = LSIGF(phi, S, x) + bias is b200gf_forward / b200gf_backward on the
+ * plan of S).  Node-major only.  For every edge feature e of `plan`, with S~_e = S_e - diag(S_e), d_e = diag(S_e) and
+ * r = 1 / (d_e - psi[f,e,p,g]) (per node), in the COLUMN convention S~ v:
+ *   z_0 = r . x_g, z_t = r . (S~_e z_{t-1}) (t = 1..tMax);   y_0 = x_g, y_t = r . (S~_e y_{t-1}) (t = 1..tMax+1)
+ *   out[n, b*F + f] += sum_{e,p,g} ( varphi[f,e,p,g] sum_t (-1)^t z_t + (-1)^(tMax+1) y_{tMax+1} )[n, b]
+ * plan: built from S~_e^T (b200gf_plan_create), so its FWD hop is S~_e v and its BWD hop S~_e^T v.
+ * d: [E, N] (the diagonals, row e for edge feature e).  psi, varphi: [F, E, P, G].  tMax >= 0.
+ *
+ * b200gf_arma_forward: x [N, x_ld] (ld >= B*G), out [N, out_ld] (ld >= B*F) is ADDED to (it normally holds the H3 term
+ *   and the bias already); nothing at or past column B*F of out is written.  states: NULL (inference: two ping-pong
+ *   states in the workspace) or a buffer of b200gf_arma_workspace_bytes(..., 3) bytes, 256-byte aligned, that receives
+ *   the E*(tMax+1) wide states [N, ldw] the backward reads (ldw = B*F*P*G*2 padded to 32 bytes).
+ * b200gf_arma_backward: dy [N, dy_ld] = dU, states = the forward's.
+ *   dx (NULL to skip) [N, dx_ld]: ADDED to, dx_g += sum_{e,f,p} r . lambda_0 + sum_e S~_e^T sum_{f,p} (r . mu_1) with the
+ *     adjoints lambda_tMax = (-1)^tMax varphi dU, lambda_t = (-1)^t varphi dU + S~^T (r . lambda_{t+1}),
+ *     mu_{tMax+1} = (-1)^(tMax+1) dU, mu_t = S~^T (r . mu_{t+1}); nothing at or past column B*G is written.
+ *   dpsi, dvarphi [F, E, P, G] (never NULL; every element written):
+ *     dpsi = sum_{n,b} ( sum_t lambda_t . r . z_t + sum_{t>=1} mu_t . r . y_t ),  dvarphi = sum_{n,b} dU sum_t (-1)^t z_t,
+ *     as deterministic two-pass column sums over fixed row pieces.
+ * workspace: b200gf_arma_workspace_bytes(plan, B, G, F, P, tMax, what) bytes, 256-byte aligned; what = 0 forward without
+ *   states, 1 forward with states, 2 backward, 3 the size of the forward's `states` buffer.  0 = invalid arguments.
+ * ---------------------------------------------------------------------------------------------- */
+int b200gf_arma_forward(const b200gf_plan* plan, const void* d, const void* psi, const void* varphi, int tMax,
+                        int B, int G, int F, int P, const void* x, int64_t x_ld, void* out, int64_t out_ld,
+                        void* states, void* workspace, size_t workspace_bytes, void* stream);
+int b200gf_arma_backward(const b200gf_plan* plan, const void* d, const void* psi, const void* varphi, int tMax,
+                         int B, int G, int F, int P, const void* dy, int64_t dy_ld, const void* states,
+                         void* dx, int64_t dx_ld, void* dpsi, void* dvarphi,
+                         void* workspace, size_t workspace_bytes, void* stream);
+size_t b200gf_arma_workspace_bytes(const b200gf_plan* plan, int B, int G, int F, int P, int tMax, int what);
+
 /* layout conversion between the reference's [C, N] (feature-major, C = B*G) and node-major [N, ld] */
 int b200gf_to_node_major(int dtype, const void* src_cn, void* dst_nc, int64_t dst_ld,
                          int64_t N, int C, void* stream);

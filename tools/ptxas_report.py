@@ -1,6 +1,8 @@
 #!/usr/bin/env python
 """nvcc -Xptxas -v output (stdin or file) -> one line per kernel: registers, stack, spill stores/loads, smem.
-   usage: nvcc ... -Xptxas -v ... 2>&1 | python tools/ptxas_report.py [filter-substring]"""
+   usage: nvcc ... -Xptxas -v ... 2>&1 | python tools/ptxas_report.py [filter-substring]
+   The library's sources are graph-neural-networks_b200/build.py's SOURCES: csrc/*.cu, csrc/nv/nv.cu and
+   csrc_arma/arma.cu (e.g. `... -c graph-neural-networks_b200/csrc_arma/arma.cu ... | python tools/ptxas_report.py arma_`)."""
 import re
 import subprocess
 import sys
@@ -31,7 +33,8 @@ try:
 except Exception:
     dem = names
 for r, d in zip(rows, dem):
-    d = re.sub(r"\(.*", "", d).replace("void b200gf::", "")
+    # kernels in an anonymous namespace (csrc/nv/nv.cu, csrc_arma/arma.cu) demangle with "(anonymous namespace)::"
+    d = re.sub(r"\(.*", "", d.replace("(anonymous namespace)::", "")).replace("void b200gf::", "").replace("void ", "")
     if flt and flt not in d:
         continue
     print("%-90s regs=%3d stack=%3d spill_st=%3d spill_ld=%3d" % (d[:90], r.get("regs", -1), r.get("stack", -1), r.get("sst", -1), r.get("sld", -1)))
