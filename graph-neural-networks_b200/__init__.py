@@ -14,6 +14,8 @@ from .recurrent import GatedGRNN, HiddenState, TimeGatedHiddenState, NodeGatedHi
 from .edgegated import EdgeGatedGRNN, EdgeGatedHiddenState, EdgeGatePattern  # noqa: F401,E402
 from .nodevariant import NVGF, NodeVariantGF, TapMap, copy_nodes  # noqa: F401,E402
 from .arma import jARMA, GraphFilterARMA, ArmaOperator  # noqa: F401,E402
+from .attention import (graphAttention, graphAttentionLSIGF, graphAttentionEVGF, GraphAttentional,  # noqa: F401,E402
+                        GraphFilterAttentional, EdgeVariantAttentional)
 from .delayed import LSIGF_DB, GraphFilter_DB, GRNN_DB, HiddenState_DB  # noqa: F401,E402
 from .graphed import graphed, GraphedForward  # noqa: F401,E402
 

@@ -65,6 +65,9 @@ _SIGNATURES = {
     "b200gf_egate_attention_forward": (c_int, [c_int, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200gf_egate_attention_backward": (c_int, [c_int, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                                 c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b200gf_attention_forward": (c_int, [c_int, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b200gf_attention_backward": (c_int, [c_int, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                          c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200gf_gated_hop_forward": (c_int, [c_int, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp,
                                          c_i64, c_vp, c_i64, c_vp]),
     "b200gf_gated_hop_backward": (c_int, [c_int, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,

@@ -5,6 +5,8 @@
 // Everything it needs lives on the non-zeros of S + I, so the kernels here work per non-zero:
 //
 //   attention  alpha[q, b] = softmax over the mask row i of  LeakyReLU_0.2(a1 s[j, b] + a2 s[i, b]),   q = (i, j)
+//              (the graph attention layers, attention.py, score the two ends with two arrays and the mixer (1, 1):
+//               LeakyReLU_0.2(s_src[j, b] + s_dst[i, b]), b200gf_attention_forward / _backward)
 //              mask = |S + I| > 1e-9 (graphML.py:692, :726-728), a = the gate's mixer, s = W z_gate (one scalar per
 //              node and sample).  The FIRST mixer half multiplies the COLUMN node j (graphML.py:706-712).
 //   gated hop  dst[j, (b, c)] = sum_i S_ij alpha[b, p(i, j)] src[i, (b, c)]         row-vector shift u S~, S~ = alpha (.) S
@@ -27,10 +29,13 @@ __device__ __forceinline__ T leaky(T v) { return v > T(0) ? v : T(0.2) * v; }
 __device__ __forceinline__ float ex(float v) { return expf(v); }
 __device__ __forceinline__ double ex(double v) { return exp(v); }
 
-// one thread per (mask row i, sample b): three passes over the row (max, exp + sum, scale)
+// one thread per (mask row i, sample b): three passes over the row (max, exp + sum, scale).  s_src is read at the
+// column node j, s_dst at the row node i (edge gating passes its one score array as both; the graph attention layers
+// pass the mixer (1, 1), so that their logit is s_src[j] + s_dst[i])
 template <typename T>
 __global__ __launch_bounds__(256) void egate_softmax_kernel(const int64_t* __restrict__ rowptr,
-                                                            const int32_t* __restrict__ col, const T* __restrict__ s,
+                                                            const int32_t* __restrict__ col,
+                                                            const T* __restrict__ s_src, const T* __restrict__ s_dst,
                                                             const T* __restrict__ mixer, T* __restrict__ alpha, int Bs,
                                                             int64_t total /* N * Bs */) {
   const T a1 = mixer[0], a2 = mixer[1];
@@ -39,12 +44,12 @@ __global__ __launch_bounds__(256) void egate_softmax_kernel(const int64_t* __res
     const int64_t i = t / Bs;
     const int64_t beg = rowptr[i], end = rowptr[i + 1];
     if (beg == end) continue;
-    const T si = a2 * s[i * Bs + b];
+    const T si = a2 * s_dst[i * Bs + b];
     T m = -INFINITY;
-    for (int64_t q = beg; q < end; ++q) m = fmax(m, leaky(a1 * s[(int64_t)col[q] * Bs + b] + si));
+    for (int64_t q = beg; q < end; ++q) m = fmax(m, leaky(a1 * s_src[(int64_t)col[q] * Bs + b] + si));
     T sum = T(0);
     for (int64_t q = beg; q < end; ++q) {
-      const T w = ex(leaky(a1 * s[(int64_t)col[q] * Bs + b] + si) - m);
+      const T w = ex(leaky(a1 * s_src[(int64_t)col[q] * Bs + b] + si) - m);
       alpha[q * Bs + b] = w;
       sum += w;
     }
@@ -57,7 +62,8 @@ __global__ __launch_bounds__(256) void egate_softmax_kernel(const int64_t* __res
 //   dlogit[q] = alpha[q] (dalpha[q] - sum_row alpha dalpha) * LeakyReLU'(e[q]);   dsig2[i] = sum_row dlogit
 template <typename T>
 __global__ __launch_bounds__(256) void egate_softmax_bwd_kernel(const int64_t* __restrict__ rowptr,
-                                                                const int32_t* __restrict__ col, const T* __restrict__ s,
+                                                                const int32_t* __restrict__ col,
+                                                                const T* __restrict__ s_src, const T* __restrict__ s_dst,
                                                                 const T* __restrict__ mixer, const T* __restrict__ alpha,
                                                                 const T* __restrict__ dalpha, T* __restrict__ dlogit,
                                                                 T* __restrict__ dsig2, int Bs, int64_t total) {
@@ -68,11 +74,11 @@ __global__ __launch_bounds__(256) void egate_softmax_bwd_kernel(const int64_t* _
     const int64_t beg = rowptr[i], end = rowptr[i + 1];
     T dot = T(0);
     for (int64_t q = beg; q < end; ++q) dot = fma(alpha[q * Bs + b], dalpha[q * Bs + b], dot);
-    const T si = a2 * s[i * Bs + b];
+    const T si = a2 * s_dst[i * Bs + b];
     T acc = T(0);
     for (int64_t q = beg; q < end; ++q) {
       const T de = alpha[q * Bs + b] * (dalpha[q * Bs + b] - dot);
-      const T dl = a1 * s[(int64_t)col[q] * Bs + b] + si > T(0) ? de : T(0.2) * de;
+      const T dl = a1 * s_src[(int64_t)col[q] * Bs + b] + si > T(0) ? de : T(0.2) * de;
       dlogit[q * Bs + b] = dl;
       acc += dl;
     }
@@ -185,23 +191,23 @@ __global__ __launch_bounds__(256) void egate_sddmm_kernel(const int64_t* __restr
 inline int grid_for(int64_t total) { return (int)imin64((total + 255) / 256, 132 * 16); }
 
 template <typename T>
-int attention_forward_t(int64_t N, int Bs, const int64_t* rowptr, const int32_t* col, const T* s, const T* mixer,
-                        T* alpha, cudaStream_t st) {
+int attention_forward_t(int64_t N, int Bs, const int64_t* rowptr, const int32_t* col, const T* s_src, const T* s_dst,
+                        const T* mixer, T* alpha, cudaStream_t st) {
   const int64_t total = N * Bs;
   if (total == 0) return B200GF_OK;
-  egate_softmax_kernel<T><<<grid_for(total), 256, 0, st>>>(rowptr, col, s, mixer, alpha, Bs, total);
+  egate_softmax_kernel<T><<<grid_for(total), 256, 0, st>>>(rowptr, col, s_src, s_dst, mixer, alpha, Bs, total);
   LAUNCH_CHECK();
   return B200GF_OK;
 }
 
 template <typename T>
 int attention_backward_t(int64_t N, int Bs, const int64_t* rowptr, const int32_t* col, const int64_t* rowptrT,
-                         const int32_t* permT, const T* s, const T* mixer, const T* alpha, const T* dalpha, T* dlogit,
-                         T* dsig1, T* dsig2, cudaStream_t st) {
+                         const int32_t* permT, const T* s_src, const T* s_dst, const T* mixer, const T* alpha,
+                         const T* dalpha, T* dlogit, T* dsig1, T* dsig2, cudaStream_t st) {
   const int64_t total = N * Bs;
   if (total == 0) return B200GF_OK;
-  egate_softmax_bwd_kernel<T><<<grid_for(total), 256, 0, st>>>(rowptr, col, s, mixer, alpha, dalpha, dlogit, dsig2, Bs,
-                                                               total);
+  egate_softmax_bwd_kernel<T><<<grid_for(total), 256, 0, st>>>(rowptr, col, s_src, s_dst, mixer, alpha, dalpha, dlogit,
+                                                               dsig2, Bs, total);
   LAUNCH_CHECK();
   egate_colsum_kernel<T><<<grid_for(total), 256, 0, st>>>(rowptrT, permT, dlogit, dsig1, Bs, total);
   LAUNCH_CHECK();
@@ -264,10 +270,11 @@ int b200gf_egate_attention_forward(int dtype, int64_t N, int64_t nnz, int Bs, co
   if (N > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == B200GF_F32)
-    return egate::attention_forward_t<float>(N, Bs, rowptr, col, (const float*)s, (const float*)mixer, (float*)alpha, st);
+    return egate::attention_forward_t<float>(N, Bs, rowptr, col, (const float*)s, (const float*)s, (const float*)mixer,
+                                             (float*)alpha, st);
   if (dtype == B200GF_F64)
-    return egate::attention_forward_t<double>(N, Bs, rowptr, col, (const double*)s, (const double*)mixer, (double*)alpha,
-                                              st);
+    return egate::attention_forward_t<double>(N, Bs, rowptr, col, (const double*)s, (const double*)s,
+                                              (const double*)mixer, (double*)alpha, st);
   return B200GF_EUNSUPPORTED;
 }
 
@@ -282,13 +289,51 @@ int b200gf_egate_attention_backward(int dtype, int64_t N, int64_t nnz, int Bs, c
   if (N > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == B200GF_F32)
-    return egate::attention_backward_t<float>(N, Bs, rowptr, col, rowptrT, permT, (const float*)s, (const float*)mixer,
-                                              (const float*)alpha, (const float*)dalpha, (float*)dlogit, (float*)dsig1,
+    return egate::attention_backward_t<float>(N, Bs, rowptr, col, rowptrT, permT, (const float*)s, (const float*)s,
+                                              (const float*)mixer, (const float*)alpha, (const float*)dalpha, (float*)dlogit, (float*)dsig1,
                                               (float*)dsig2, st);
   if (dtype == B200GF_F64)
     return egate::attention_backward_t<double>(N, Bs, rowptr, col, rowptrT, permT, (const double*)s,
-                                               (const double*)mixer, (const double*)alpha, (const double*)dalpha,
+                                               (const double*)s, (const double*)mixer, (const double*)alpha, (const double*)dalpha,
                                                (double*)dlogit, (double*)dsig1, (double*)dsig2, st);
+  return B200GF_EUNSUPPORTED;
+}
+
+int b200gf_attention_forward(int dtype, int64_t N, int64_t nnz, int Bs, const int64_t* rowptr, const int32_t* col,
+                             const void* s_src, const void* s_dst, const void* mixer, void* alpha, void* stream) {
+  using namespace b200gf;
+  if (N < 0 || nnz < 0 || Bs <= 0) return B200GF_EINVAL;
+  if (!rowptr || !s_src || !s_dst || !mixer || (nnz > 0 && (!col || !alpha))) return B200GF_EINVAL;
+  if (N > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == B200GF_F32)
+    return egate::attention_forward_t<float>(N, Bs, rowptr, col, (const float*)s_src, (const float*)s_dst,
+                                             (const float*)mixer, (float*)alpha, st);
+  if (dtype == B200GF_F64)
+    return egate::attention_forward_t<double>(N, Bs, rowptr, col, (const double*)s_src, (const double*)s_dst,
+                                              (const double*)mixer, (double*)alpha, st);
+  return B200GF_EUNSUPPORTED;
+}
+
+int b200gf_attention_backward(int dtype, int64_t N, int64_t nnz, int Bs, const int64_t* rowptr, const int32_t* col,
+                              const int64_t* rowptrT, const int32_t* permT, const void* s_src, const void* s_dst,
+                              const void* mixer, const void* alpha, const void* dalpha, void* dlogit, void* dsig1, void* dsig2,
+                              void* stream) {
+  using namespace b200gf;
+  if (N < 0 || nnz < 0 || Bs <= 0) return B200GF_EINVAL;
+  if (!rowptr || !rowptrT || !s_src || !s_dst || !mixer || !dsig1 || !dsig2) return B200GF_EINVAL;
+  if (nnz > 0 && (!col || !permT || !alpha || !dalpha || !dlogit)) return B200GF_EINVAL;
+  if (N > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == B200GF_F32)
+    return egate::attention_backward_t<float>(N, Bs, rowptr, col, rowptrT, permT, (const float*)s_src,
+                                              (const float*)s_dst, (const float*)mixer, (const float*)alpha, (const float*)dalpha,
+                                              (float*)dlogit, (float*)dsig1, (float*)dsig2, st);
+  if (dtype == B200GF_F64)
+    return egate::attention_backward_t<double>(N, Bs, rowptr, col, rowptrT, permT, (const double*)s_src,
+                                               (const double*)s_dst, (const double*)mixer, (const double*)alpha,
+                                               (const double*)dalpha, (double*)dlogit, (double*)dsig1, (double*)dsig2,
+                                               st);
   return B200GF_EUNSUPPORTED;
 }
 

@@ -45,50 +45,72 @@ def _rowptr(rows, N):
 
 
 class EdgeGatePattern:
-    """Sparse structure of one edge-gated layer's GSO S (E = 1).
+    """Sparse structure of a GSO S [E, N, N] for the edge-gated layer (E = 1) and the graph attention layers (E >= 1).
 
-    `EdgeGatePattern(S)`: S a dense [1, N, N] tensor (built on S's device) or a SparseGSO (built from its CSR on the
+    `EdgeGatePattern(S)`: S a dense [E, N, N] tensor (built on S's device) or a SparseGSO (built from its CSR on the
     host; never densified).  `on(device)` returns the pattern on another device (cached).  Members (int64 offsets,
     int32 indices):
-      mask CSR of |S + I| > 1e-9 (graphML.py:692, :726-728):  m_rowptr, m_col (ascending), m_row; nnz = its size
+      mask CSR, one for all edge features (graphML.py:692, :726-728): off the diagonal sum_e |S_e,ij| > 1e-9, on it
+        sum_e |S_e,ii + 1| > 1e-9:  m_rowptr, m_col (ascending), m_row; nnz = its size
       its transpose:  mT_rowptr, mT_perm (position in the mask of the k-th entry of column j)
       CSR of S^T:     t_rowptr, t_col (= i), t_val (= S_ij), t_pos (= p(i, j) in the mask, -1 outside it)
       CSR of S:       s_rowptr, s_col (= j), s_val, s_pos
-      m_sval:         S_ij in mask order (0 where S has no entry, e.g. the diagonal added by + I)."""
+      m_sval:         S_ij in mask order (0 where S has no entry, e.g. the diagonal added by + I).
+    The t_*, s_* and m_sval members are those of edge feature 0; `edges[e]` is a pattern holding edge feature e's (it
+    shares the mask members; edges[0] is the pattern itself).  `unit()` is the mask itself with unit values (the hop by
+    alpha alone of GraphFilterAttentional)."""
 
     def __init__(self, S=None):
         self._devices = {}
         self._vals = {}
+        self._unit = None
         if S is None:
             return
-        assert len(S.shape) == 3 and S.shape[0] == 1, "edge gating runs on one edge feature (graphML.py:4190-4197)"
-        N = int(S.shape[1])
-        if isinstance(S, SparseGSO):
-            rowptr, col, val = S.csr[0]
-            rows = torch.from_numpy(np.repeat(np.arange(N, dtype=np.int64), np.diff(rowptr)))
-            cols = torch.from_numpy(col.astype(np.int64))
-            vals = torch.from_numpy(np.ascontiguousarray(val))
-            keep = vals != 0
-            rows, cols, vals = rows[keep], cols[keep], vals[keep]
-        else:
-            nz = (S[0] != 0).nonzero(as_tuple=False)                # row-major
-            rows, cols = nz[:, 0], nz[:, 1]
-            vals = S[0][rows, cols]
-        self._build(N, rows, cols, vals.detach())
+        assert len(S.shape) == 3
+        E, N = int(S.shape[0]), int(S.shape[1])
+        entries = []
+        for e in range(E):
+            if isinstance(S, SparseGSO):
+                rowptr, col, val = S.csr[e]
+                rows = torch.from_numpy(np.repeat(np.arange(N, dtype=np.int64), np.diff(rowptr)))
+                cols = torch.from_numpy(col.astype(np.int64))
+                vals = torch.from_numpy(np.ascontiguousarray(val))
+                keep = vals != 0
+                rows, cols, vals = rows[keep], cols[keep], vals[keep]
+            else:
+                nz = (S[e] != 0).nonzero(as_tuple=False)            # row-major
+                rows, cols = nz[:, 0], nz[:, 1]
+                vals = S[e][rows, cols]
+            entries.append((rows, cols, vals.detach()))
+        self._build(N, entries)
 
-    def _build(self, N, rows, cols, vals):
+    def _build(self, N, entries):
+        rows, cols, vals = entries[0]
         dev = rows.device
+        E = len(entries)
         self.N = N
+        self.E = E
         self.dtype = vals.dtype
-        key = rows * N + cols
-        # mask: off-diagonal entries with |S_ij| > tol, the diagonal where |S_ii + 1| > tol (so S_ii = -1 drops out)
-        diag = torch.zeros(N, dtype=vals.dtype, device=dev)
-        on = rows == cols
-        diag[rows[on]] = vals[on]
+        # mask: off-diagonal entries with sum_e |S_e,ij| > tol, the diagonal where sum_e |S_e,ii + 1| > tol (so S_ii = -1
+        # drops out when E = 1).  The sums run over a dense [E, .] stack in e order, as the reference's sum over dim 0.
         idx = torch.arange(N, device=dev)
-        off = (rows != cols) & (vals.abs() > zeroTolerance)
-        dkeep = (diag + 1).abs() > zeroTolerance
-        m_key, _ = torch.sort(torch.cat((key[off], idx[dkeep] * (N + 1))))
+        diag = torch.zeros((E, N), dtype=vals.dtype, device=dev)
+        off_keys = []
+        for e, (r, c, v) in enumerate(entries):
+            on = r == c
+            diag[e, r[on]] = v[on]
+            off_keys.append(r[~on] * N + c[~on])
+        uk, inv = torch.unique(torch.cat(off_keys), sorted=True, return_inverse=True)
+        absum = torch.zeros((E, uk.numel()), dtype=vals.dtype, device=dev)
+        o = 0
+        for e, (r, c, v) in enumerate(entries):
+            off = r != c
+            n = int(off.sum())
+            absum[e, inv[o:o + n]] = v[off].abs()
+            o += n
+        okeep = absum.sum(0) > zeroTolerance
+        dkeep = (diag + 1).abs().sum(0) > zeroTolerance
+        m_key, _ = torch.sort(torch.cat((uk[okeep], idx[dkeep] * (N + 1))))
         m_row, m_col = m_key // N, m_key % N
         nnz = int(m_key.numel())
         self.nnz = nnz
@@ -98,7 +120,16 @@ class EdgeGatePattern:
         permT = torch.argsort(m_col * N + m_row)
         self.mT_rowptr = _rowptr(m_col, N)
         self.mT_perm = permT.to(torch.int32)
-        # each S entry's position in the mask
+        self.edges = [self]
+        for e, (r, c, v) in enumerate(entries):
+            (self if e == 0 else self._child())._set_edge(N, m_key, r, c, v)
+        self.device = torch.device(dev)
+        self._devices[str(self.device)] = self
+
+    def _set_edge(self, N, m_key, rows, cols, vals):
+        """The members of one edge feature: each S_e entry's position in the mask, the CSRs of S_e and S_e^T."""
+        dev, nnz = rows.device, self.nnz
+        key = rows * N + cols
         if nnz > 0:
             pos = torch.searchsorted(m_key, key)
             hit = m_key[pos.clamp(max=nnz - 1)] == key
@@ -119,11 +150,26 @@ class EdgeGatePattern:
         self.t_col = rows[oT].to(torch.int32)
         self.t_val = vals[oT]
         self.t_pos = pos[oT].to(torch.int32)
-        self.device = torch.device(dev)
-        self._devices[str(self.device)] = self
 
+    @property
+    def shape(self):
+        """(E, N, N), as the GSO's: the attention functionals take a pattern where the reference takes S."""
+        return (self.E, self.N, self.N)
+
+    _MASK = ("m_rowptr", "m_col", "m_row", "mT_rowptr", "mT_perm")
     _TENSORS = ("m_rowptr", "m_col", "m_row", "mT_rowptr", "mT_perm", "m_sval", "s_rowptr", "s_col", "s_val", "s_pos",
                 "t_rowptr", "t_col", "t_val", "t_pos")
+
+    def _child(self):
+        """An empty pattern sharing this one's mask (to receive another edge feature's members)."""
+        c = EdgeGatePattern()
+        c.N, c.E, c.nnz, c.dtype = self.N, 1, self.nnz, self.dtype
+        c.device = getattr(self, "device", None)
+        for name in self._MASK:
+            setattr(c, name, getattr(self, name))
+        c.edges = [c]
+        self.edges.append(c)
+        return c
 
     def on(self, device):
         device = torch.device(device)
@@ -132,12 +178,35 @@ class EdgeGatePattern:
         hit = self._devices.get(str(device))
         if hit is None:
             hit = EdgeGatePattern()
-            hit.N, hit.nnz, hit.dtype, hit.device = self.N, self.nnz, self.dtype, device
+            hit.N, hit.E, hit.nnz, hit.dtype, hit.device = self.N, self.E, self.nnz, self.dtype, device
             for name in self._TENSORS:
                 setattr(hit, name, getattr(self, name).to(device))
+            hit.edges = [hit]
+            for src in self.edges[1:]:
+                c = hit._child()
+                for name in self._TENSORS[len(self._MASK):]:
+                    setattr(c, name, getattr(src, name).to(device))
             hit._devices = self._devices
             self._devices[str(device)] = hit
         return hit
+
+    def unit(self):
+        """The mask as a hop operator with unit values (cached): the CSR of its transpose for the forward hop, the mask
+        CSR for the backward one, every entry at its own mask position."""
+        if self._unit is None:
+            u = EdgeGatePattern()
+            u.N, u.E, u.nnz, u.dtype, u.device = self.N, 1, self.nnz, self.dtype, self.device
+            for name in self._MASK:
+                setattr(u, name, getattr(self, name))
+            ones = torch.ones(self.nnz, dtype=self.dtype, device=self.m_col.device)
+            u.m_sval = ones
+            u.s_rowptr, u.s_col, u.s_val = self.m_rowptr, self.m_col, ones
+            u.s_pos = torch.arange(self.nnz, dtype=torch.int32, device=self.m_col.device)
+            u.t_rowptr, u.t_col, u.t_val = self.mT_rowptr, self.m_row[self.mT_perm.long()].to(torch.int32), ones
+            u.t_pos = self.mT_perm
+            u.edges = [u]
+            self._unit = u
+        return self._unit
 
     def values(self, dtype):
         """(t_val, s_val, m_sval) in the compute dtype (cached)."""

@@ -330,19 +330,23 @@ def fuse_layers(model):
 _SAVED = {}
 
 
-def install(gml=None, edge_gating=False, node_variant=False, arma=False):
+def install(gml=None, edge_gating=False, node_variant=False, arma=False, attention=False):
     """Point `alegnn.utils.graphML.LSIGF`, `.GraphFilter`, `.EVGF`, `.EdgeVariantGF`, the local pooling / activation
     layers and the static-GSO recurrent layers at this package.  `edge_gating=True` also points
     `.EdgeGatedHiddenState` at the sparse edge-gated layer (edgegated.py); by default it stays the reference's.
     `node_variant=True` also points `.NVGF` and `.NodeVariantGF` at the sparse node-variant filter (nodevariant.py);
     by default they stay the reference's.  `arma=True` also points `.jARMA` and `.GraphFilterARMA` at the sparse ARMA
     filter (arma.py); by default they stay the reference's (whose residue term still runs on this package's LSIGF).
+    `attention=True` also points `.GraphAttentional`, `.GraphFilterAttentional`, `.EdgeVariantAttentional` and the
+    functionals `.graphAttention`, `.graphAttentionLSIGF`, `.graphAttentionEVGF` at the sparse attention layers
+    (attention.py); by default they stay the reference's.  `.learnAttentionGSO`, which returns a dense tensor, is always
+    the reference's.
 
     `GraphFilter.forward` in the reference looks `LSIGF` up as a module global at call time (graphML.py:2137), so
     this also accelerates its hybrid EdgeVariantGF (:2686), jARMA (:592) and GatedGRNN (:1403,:1461) call sites.
     Architectures built AFTER install() get this package's layers (plan cached in addGSO).
     """
-    from . import activations, arma as arma_mod, delayed, edgegated, edgevariant, nodevariant, pooling, recurrent
+    from . import activations, arma as arma_mod, attention as attention_mod, delayed, edgegated, edgevariant, nodevariant, pooling, recurrent
     if gml is None:
         import alegnn.utils.graphML as gml
     if id(gml) not in _SAVED:
@@ -368,6 +372,14 @@ def install(gml=None, edge_gating=False, node_variant=False, arma=False):
         # sparse Jacobi chains on the S~ plan instead of [F,E,P,G,N,N] dense operators (arma.py)
         gml.jARMA = arma_mod.jARMA
         gml.GraphFilterARMA = arma_mod.GraphFilterARMA
+    if attention:
+        names = ("graphAttention", "graphAttentionLSIGF", "graphAttentionEVGF", "GraphAttentional",
+                 "GraphFilterAttentional", "EdgeVariantAttentional")
+        for name in names:
+            _SAVED[id(gml)][1].setdefault(name, getattr(gml, name))
+        # attention per non-zero of the mask of S + I and gated sparse hops instead of B x P x E x N x N tensors
+        for name in names:
+            setattr(gml, name, getattr(attention_mod, name))
     gml.LSIGF = LSIGF
     gml.GraphFilter = GraphFilter
     gml.EVGF = edgevariant.EVGF

@@ -321,6 +321,22 @@ int b200gf_egate_attention_backward(int dtype, int64_t N, int64_t nnz, int Bs,
                                     const int64_t* rowptrT, const int32_t* permT,
                                     const void* s, const void* mixer, const void* alpha, const void* dalpha,
                                     void* dlogit, void* dsig1, void* dsig2, void* stream);
+/* Graph attention layers (GraphAttentional, GraphFilterAttentional, EdgeVariantAttentional, graphML.py:739-969,
+ * :2849-3270): the same attention on the same mask CSR, with the two ends of an edge scored by two arrays, s_src read at
+ * the column node j and s_dst at the row node i (mixer: DEVICE pointer to (a1, a2); the layers pass (1, 1)):
+ *   forward:  alpha[q, b] = softmax over the mask row i of LeakyReLU_0.2(a1 s_src[j, b] + a2 s_dst[i, b]), q = (i, j);
+ *   backward: dlogit as above; dsig1[j, b] = sum over column j of dlogit (the gradient of the a1 s_src term),
+ *             dsig2[i, b] = sum over row i of dlogit (of the a2 s_dst term).
+ * s_src, s_dst, dsig1, dsig2 [N, Bs]; alpha, dalpha, dlogit [nnz, Bs].  b200gf_egate_attention_* are these with s
+ * passed as both arrays. */
+int b200gf_attention_forward(int dtype, int64_t N, int64_t nnz, int Bs,
+                             const int64_t* rowptr, const int32_t* col,
+                             const void* s_src, const void* s_dst, const void* mixer, void* alpha, void* stream);
+int b200gf_attention_backward(int dtype, int64_t N, int64_t nnz, int Bs,
+                              const int64_t* rowptr, const int32_t* col,
+                              const int64_t* rowptrT, const int32_t* permT,
+                              const void* s_src, const void* s_dst, const void* mixer, const void* alpha,
+                              const void* dalpha, void* dlogit, void* dsig1, void* dsig2, void* stream);
 int b200gf_gated_hop_forward(int dtype, int64_t N, int Bs, int C,
                              const int64_t* rowptrT, const int32_t* colT, const void* valT, const int32_t* posT,
                              const void* gate, int64_t gate_sb, int64_t gate_sp,
