@@ -1,4 +1,4 @@
-"""ARMA graph filters by Jacobi iterations on sparse CUDA kernels (csrc_arma/arma.cu).
+"""ARMA graph filters by Jacobi iterations on sparse CUDA kernels (csrc/arma/arma.cu).
 
     jARMA(psi, varphi, phi, S, x, b=None, tMax=5)        <- alegnn/utils/graphML.py:490-638
     GraphFilterARMA(G, F, P, K, E=1, bias=True, tMax=5)   <- graphML.py:2714-2847  (same attributes, parameter names

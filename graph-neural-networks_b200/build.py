@@ -12,9 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200gf.so")
 SOURCES = ["plan.cu", "spmm.cu", "taps.cu", "layout.cu", "lsigf.cu", "tc_contract.cu", "ev.cu", "layer.cu", "dmma_contract.cu",
-           "egate.cu", "nv/nv.cu",
-           # beside csrc/, not under it: see the header of csrc_arma/arma.cu
-           "../csrc_arma/arma.cu"]
+           "egate.cu", "nv/nv.cu", "arma/arma.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-O3,-Wall", "--expt-relaxed-constexpr"]
 
@@ -33,8 +31,11 @@ def _stale(target, deps):
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build_library(force=False, verbose=False, extra_sources=()):
-    srcs = [os.path.join(CSRC, s) for s in list(SOURCES) + list(extra_sources) if os.path.exists(os.path.join(CSRC, s))]
+def build_library(force=False, verbose=False):
+    srcs = [os.path.join(CSRC, s) for s in SOURCES]
+    missing = [s for s in srcs if not os.path.exists(s)]
+    if missing:
+        raise FileNotFoundError("b200gf: listed CUDA sources do not exist: %s" % ", ".join(missing))
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     headers.append(os.path.join(os.path.dirname(HERE), "include", "b200gf.h"))
     objdir = os.path.join(HERE, "build")

@@ -1,4 +1,4 @@
-"""ARMA graph filters (gnn_b200.arma, csrc_arma/arma.cu) against fixtures produced by the unmodified reference
+"""ARMA graph filters (gnn_b200.arma, csrc/arma/arma.cu) against fixtures produced by the unmodified reference
 (tests/golden/arma_cases.npz <- oracle/make_golden_arma.py: jARMA, alegnn/utils/graphML.py:490-638; GraphFilterARMA
 :2714-2847; ARMAfilterGNN, alegnn/modules/architectures.py:2243-2555).
 

@@ -1,36 +1,22 @@
-"""One case per launch branch of the ARMA filter's kernels (csrc_arma/arma.cu), each held to oracle/arma_oracle.py's
-componentwise fp64 bound, in the format of tests/test_nv_dispatch.py and with tests/test_kernel_dispatch.py's helpers.
+"""One case per launch branch of the ARMA filter's kernels (csrc/arma/arma.cu), each held to oracle/arma_oracle.py's
+componentwise fp64 bound by tests/dispatch_harness.py's check_case.  This table owns the kernels of csrc/arma/
+(tests/test_dispatch_tables.py).
 
 Every row calls b200gf_arma_forward (with saved states, and without: the inference ping-pong) and b200gf_arma_backward
-through the C ABI and names the kernels its branch must launch.  The rows' launches are traced in a child process, as
-tests/test_egate_dispatch.py does, so this table's profiling leaves the pytest process's profiler untouched.  Outputs
+through the C ABI and names the kernels its branch must launch.  The rows' launches are traced in a child process
+(dispatch_harness.child_traced), so this table's profiling leaves the pytest process's profiler untouched.  Outputs
 are checked against their bound; memory outside the contract must keep its canary pattern; NaN in input pad columns
 must reach no output; a rerun must be bit-identical; and the inference forward must equal the training forward bit for
-bit.  The CPU tests keep all three kernel tables honest: every __global__ function anywhere in the package (csrc/,
-csrc/nv/, csrc_arma/) has a case in this table, test_nv_dispatch.py's or test_kernel_dispatch.py's (or is excluded
-there), so no kernel escapes coverage by sitting outside csrc/.
+bit.
 """
-import glob
-import json
-import os
-import re
-import shutil
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import scipy.sparse as sp
 import torch
 
 import lsigf_oracle as orc
-import test_kernel_dispatch as kd
-import test_nv_dispatch as nvd
-from test_egate_dispatch import _profiled
-from test_kernel_dispatch import F32, F64, NPD, SENT, Result, _check, _from_node_major, _graph, _lib, _st
-
-PKG = os.path.dirname(kd.CSRC)
-ARMA_DIR = os.path.join(PKG, "csrc_arma")
+from dispatch_harness import (F32, F64, NPD, SENT, Result, _check, _from_node_major, _graph, _lib, _st, check_case,
+                              child_traced)
 
 
 def _arma_case(dtype, N, B, G, F, P, E, tMax, graph="rand", x_pad=3, diag="vary"):
@@ -157,55 +143,6 @@ ARMA_CASES = _arma_rows()
 
 
 # ------------------------------------------------------------------------------------------------------------ CPU
-def _package_global_functions():
-    """(path relative to the package, kernel) for every __global__ function in any .cu / .cuh of the package."""
-    out = set()
-    for path in glob.glob(os.path.join(PKG, "**", "*.cu"), recursive=True) + \
-            glob.glob(os.path.join(PKG, "**", "*.cuh"), recursive=True):
-        src = open(path).read()
-        for name in re.findall(r"__global__\s+(?:__launch_bounds__\([^)]*\)\s*)?void\s+"
-                               r"(?:__launch_bounds__\([^)]*\)\s*)?(\w+)\s*\(", src):
-            out.add((os.path.relpath(path, PKG), name))
-    return out
-
-
-def test_every_global_function_in_the_package_has_a_case():
-    """Every kernel of the package is covered by one of the three tables: csrc_arma/ here, csrc/nv/ in
-    test_nv_dispatch.py, the rest of csrc/ in test_kernel_dispatch.py (a case or a listed exclusion)."""
-    found = _package_global_functions()
-    arma = {k for f, k in found if f.startswith("csrc_arma" + os.sep)}
-    assert arma, "no kernels found under csrc_arma/"
-    missing_arma = sorted(arma - nvd._covered(ARMA_CASES))
-    assert not missing_arma, "ARMA kernels without a dispatch case: %s" % missing_arma
-    stale = sorted(nvd._covered(ARMA_CASES) - arma)
-    assert not stale, "table names that are not __global__ functions in csrc_arma/: %s" % stale
-    covered = nvd._covered(ARMA_CASES) | nvd._covered(nvd.NV_CASES) | nvd._covered(kd.CASES) | set(kd.EXCLUDED)
-    missing = sorted("%s:%s" % fk for fk in found if fk[1] not in covered)
-    assert not missing, "kernels in the package without a dispatch case or an exclusion: %s" % missing
-    outside = sorted(f for f, _ in found if not f.startswith(("csrc" + os.sep, "csrc_arma" + os.sep)))
-    assert not outside, "kernels outside csrc/ and csrc_arma/: %s" % outside
-    ids = [c[0] for c in ARMA_CASES]
-    assert len(ids) == len(set(ids)) and not set(ids) & ({c[0] for c in kd.CASES} | {c[0] for c in nvd.NV_CASES})
-
-
-def test_every_expected_arma_kernel_is_instantiated_in_the_library():
-    import gnn_b200
-    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    filt = shutil.which("cu++filt") or "/usr/local/cuda/bin/cu++filt"
-    if not (os.path.exists(tool) and os.path.exists(filt)):
-        pytest.skip("cuobjdump / cu++filt not available")
-    lib = gnn_b200._cabi.LIB_PATH
-    if not os.path.exists(lib):
-        pytest.skip("library not built")
-    syms = subprocess.run([tool, "-symbols", lib], capture_output=True, text=True, check=True).stdout
-    mangled = re.findall(r"STT_FUNC\s+.*?\s(\S+)\s*$", syms, flags=re.M)
-    names = [kd._norm(n) for n in subprocess.run([filt], input="\n".join(mangled), capture_output=True, text=True,
-                                                  check=True).stdout.splitlines()]
-    for cid, _, ks in ARMA_CASES:
-        for k in ks:
-            assert any(re.search(k, n) for n in names), (cid, k)
-
-
 def test_the_abi_rejects_bad_arguments_before_any_cuda_call():
     """Null pointers, negative sizes, short leading dimensions and misaligned workspaces are EINVAL; a null plan sizes
     nothing."""
@@ -217,54 +154,10 @@ def test_the_abi_rejects_bad_arguments_before_any_cuda_call():
 
 
 # ------------------------------------------------------------------------------------------------------------ GPU
-def _trace_all(path):
-    """Writes {case id: traced names} of every row to path (JSON); run in a process of its own by `traced`."""
-    with open(path, "w") as f:
-        json.dump({cid: _profiled(fn, ks) for cid, fn, ks in ARMA_CASES}, f)
-
-
-@pytest.fixture(scope="module")
-def traced(tmp_path_factory):
-    """The kernels each row launches, traced in a fresh Python process (see test_egate_dispatch.traced)."""
-    path = tmp_path_factory.mktemp("arma_trace") / "names.json"
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    env = dict(os.environ, PYTHONDONTWRITEBYTECODE="1",
-               PYTHONPATH=os.pathsep.join([here, os.path.join(root, "oracle"), root]
-                                          + [p for p in os.environ.get("PYTHONPATH", "").split(os.pathsep) if p]))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    subprocess.run([sys.executable] + flags + ["-c", "import sys, test_arma_dispatch as t; t._trace_all(sys.argv[1])",
-                                               str(path)], env=env, cwd=root, check=True, timeout=1800)
-    with open(path) as f:
-        return json.load(f)
+traced = child_traced("test_arma_dispatch", "ARMA_CASES")
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid,fn,kernels", ARMA_CASES, ids=[c[0] for c in ARMA_CASES])
 def test_arma_dispatch(cid, fn, kernels, traced):
-    names = traced[cid]
-    print("%s: %s" % (cid, sorted(set(n.split("(")[0] for n in names if "kernel" in n))))
-    remaining = list(names)
-    for k in kernels:   # a regex listed twice must match two launches
-        hit = next((n for n in remaining if re.search(k, n)), None)
-        assert hit is not None, "%s: expected %s among %s" % (cid, k, sorted(set(n.split("(")[0] for n in names)))
-        remaining.remove(hit)
-    res1 = fn()
-    torch.cuda.synchronize()
-    worst = []
-    for name, out, ref, bound in res1.checks:
-        v = orc.bound_violation(out.detach().double().cpu().numpy(), ref, bound)
-        worst.append("%s %.3g" % (name, v))
-        assert v <= 1.0, "%s/%s: error %.3g x its bound" % (cid, name, v)
-    print("%s: worst error / bound: %s" % (cid, ", ".join(worst)))
-    for name, t in res1.canaries:
-        assert torch.equal(kd._bits(t), kd._bits(torch.full_like(t, SENT if t.is_floating_point() else 0x5A))), \
-            "%s: wrote outside its contract (%s)" % (cid, name)
-    for name, t in res1.finite:
-        assert bool(torch.isfinite(t).all()), "%s: non-finite %s (NaN in an input pad leaked)" % (cid, name)
-    for name, a, b in res1.same:
-        assert torch.equal(kd._bits(a), kd._bits(b)), "%s: %s" % (cid, name)
-    res2 = fn()
-    torch.cuda.synchronize()
-    for a, b in zip(res1.outputs, res2.outputs):
-        assert torch.equal(kd._bits(a), kd._bits(b)), "%s: two runs differ" % cid
+    check_case(cid, fn, kernels, traced[cid])

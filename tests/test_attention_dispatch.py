@@ -1,23 +1,19 @@
 """One case per launch branch of the two-score attention entry points (b200gf_attention_forward / _backward, which run
 csrc/egate.cu's softmax kernels with s_src read at the column node and s_dst at the row node), each held to
-oracle/attention_oracle.py's componentwise fp64 bound, in the format of tests/test_egate_dispatch.py and with its
-helpers.
+oracle/attention_oracle.py's componentwise fp64 bound by tests/dispatch_harness.py's check_case.  The table owns no
+kernel: it names only egate.cu's, which tests/test_egate_dispatch.py owns (tests/test_dispatch_tables.py).
 
 Every row calls the C entry points directly with the mixer (1, 1) the layers pass and names the kernels its branch
-must launch; the launches are traced with torch.profiler in a separate process (see `traced`).  Outputs start as NaN
-followed by 4 KB of SENT, which must survive.  Every output is held to attention_envelope, and a second run must be
-bit-identical.  Rows with `parity` also run the edge-gate entry point on s_src = s_dst with the same mixer and require
-the same bits: the generalised kernels compute what edge gating always computed.
+must launch; the launches are traced with torch.profiler in a child process (dispatch_harness.child_traced).  Outputs
+start as NaN followed by 4 KB of SENT, which must survive.  Every output is held to attention_envelope, and a second
+run must be bit-identical.  Rows with `parity` also run the edge-gate entry point on s_src = s_dst with the same mixer
+and require the same bits: the generalised kernels compute what edge gating always computed.
 
 Inputs sit on a coarse grid (multiples of 2^-10 in [-8, 8], or of 2^-4 in [-96, 96] for the large-logit rows), so the
 logit s_src[j] + s_dst[i] is exact in fp32 and fp64 and LeakyReLU' takes the same branch in the kernel and in the fp64
 restatement.  The masks are the union over E edge features (E = 2 rows: S_0 and a transposed, re-weighted copy).
 """
 import functools
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -29,8 +25,7 @@ import egate_oracle as ego
 import lsigf_oracle as orc
 import test_egate_dispatch as ed
 import test_egate_oracle as eo
-import test_kernel_dispatch as kd
-from test_kernel_dispatch import F32, F64, NPD, SENT, Result, _check, _lib, _st
+from dispatch_harness import F32, F64, NPD, Result, _bits, _check, _lib, _st, check_case, child_traced, kernel_names
 
 GRID = ed.GRID
 
@@ -123,7 +118,7 @@ def _attn2_case(dtype, N, Bs, graph="rand", E=2, s_kind="grid", backward=True, p
             _check(lib.b200gf_attention_forward(enum, N, nnz, Bs, d["m_rowptr"].data_ptr(), d["m_col"].data_ptr(),
                                                 s_src.data_ptr(), s_src.data_ptr(), ones.data_ptr(), t_ab.data_ptr(),
                                                 _st()))
-            assert torch.equal(kd._bits(e_ab), kd._bits(t_ab)), "edge-gate and two-score entry points differ on s_src = s_dst"
+            assert torch.equal(_bits(e_ab), _bits(t_ab)), "edge-gate and two-score entry points differ on s_src = s_dst"
         return res
     return run
 
@@ -231,60 +226,14 @@ def test_union_mask_differs_from_edge_feature_0():
 
 
 def test_every_row_names_only_egate_kernels():
-    import test_nv_dispatch as nvd
-    found = {k for f, k in nvd._all_global_functions() if f == "egate.cu"}
-    covered = nvd._covered(ATTENTION_CASES)
-    assert covered <= found and covered == {"egate_softmax_kernel", "egate_softmax_bwd_kernel", "egate_colsum_kernel"}
-    ids = [c[0] for c in ATTENTION_CASES]
-    assert len(ids) == len(set(ids)) and not set(ids) & {c[0] for c in ed.EGATE_CASES}
+    assert kernel_names(ATTENTION_CASES) == {"egate_softmax_kernel", "egate_softmax_bwd_kernel", "egate_colsum_kernel"}
 
 
 # ------------------------------------------------------------------------------------------------------------ GPU
-def _trace_all(path):
-    with open(path, "w") as f:
-        json.dump({cid: ed._profiled(fn, ks) for cid, fn, ks in ATTENTION_CASES}, f)
-
-
-@pytest.fixture(scope="module")
-def traced(tmp_path_factory):
-    """The kernels each row launches, traced in a fresh Python process (see test_egate_dispatch.traced)."""
-    path = tmp_path_factory.mktemp("attention_trace") / "names.json"
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    env = dict(os.environ, PYTHONDONTWRITEBYTECODE="1",
-               PYTHONPATH=os.pathsep.join([here, os.path.join(root, "oracle"), root]
-                                          + [p for p in os.environ.get("PYTHONPATH", "").split(os.pathsep) if p]))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    subprocess.run([sys.executable] + flags + ["-c", "import sys, test_attention_dispatch as t; t._trace_all(sys.argv[1])",
-                                               str(path)], env=env, cwd=root, check=True, timeout=1800)
-    with open(path) as f:
-        return json.load(f)
+traced = child_traced("test_attention_dispatch", "ATTENTION_CASES")
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid,fn,kernels", ATTENTION_CASES, ids=[c[0] for c in ATTENTION_CASES])
 def test_attention_dispatch(cid, fn, kernels, traced):
-    import re
-    names = traced[cid]
-    remaining = list(names)
-    for k in kernels:
-        hit = next((n for n in remaining if re.search(k, n)), None)
-        assert hit is not None, "%s: expected %s among %s" % (cid, k, sorted(set(n.split("(")[0] for n in names)))
-        remaining.remove(hit)
-    res1 = fn()
-    torch.cuda.synchronize()
-    worst = []
-    for name, out, ref, bound in res1.checks:
-        v = orc.bound_violation(out.detach().double().cpu().numpy(), ref, bound)
-        worst.append("%s %.3g" % (name, v))
-        assert v <= 1.0, "%s/%s: error %.3g x its bound" % (cid, name, v)
-    print("%s: worst error / bound: %s" % (cid, ", ".join(worst)))
-    for name, t in res1.canaries:
-        assert torch.equal(kd._bits(t), kd._bits(torch.full_like(t, SENT))), "%s: wrote outside its contract (%s)" % (
-            cid, name)
-    for name, t in res1.finite:
-        assert bool(torch.isfinite(t).all()), "%s: non-finite %s" % (cid, name)
-    res2 = fn()
-    torch.cuda.synchronize()
-    for a, b in zip(res1.outputs, res2.outputs):
-        assert torch.equal(kd._bits(a), kd._bits(b)), "%s: two runs differ" % cid
+    check_case(cid, fn, kernels, traced[cid])

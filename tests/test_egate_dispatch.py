@@ -1,10 +1,12 @@
 """One case per launch branch of the edge-gated layer's kernels (csrc/egate.cu), each held to oracle/egate_oracle.py's
-componentwise fp64 bound, in the format of tests/test_kernel_dispatch.py and with its helpers.
+componentwise fp64 bound by tests/dispatch_harness.py's check_case.  This table owns the kernels of egate.cu
+(tests/test_dispatch_tables.py).
 
 Every row calls the C entry points directly and names the kernels its branch must launch (regexes on the demangled
-name); the launches are traced with torch.profiler in a separate process (see `traced`).  Outputs start as NaN and are followed by 4 KB of SENT; the pad columns [Bs*C, ld) of dst and dsrc start as SENT
-and must keep it, and input pad columns hold NaN, which must reach no output.  Every output is held to
-egate_envelope, and a second run must be bit-identical.
+name); the launches are traced with torch.profiler in a child process (dispatch_harness.child_traced).  Outputs start
+as NaN and are followed by 4 KB of SENT; the pad columns [Bs*C, ld) of dst and dsrc start as SENT and must keep it,
+and input pad columns hold NaN, which must reach no output.  Every output is held to egate_envelope, and a second run
+must be bit-identical.
 
 Attention inputs sit on a coarse grid (s a multiple of 2^-10 in [-8, 8], or of 2^-4 in [-96, 96] for the large-logit
 rows; mixer values with 5 significant bits), so the logit a1 s_j + a2 s_i is exact in fp32 and fp64 and LeakyReLU'
@@ -16,21 +18,13 @@ tests/test_egate_oracle.py, which checks on the CPU that an emulated correct ker
 these shapes and that emulated wrong kernels do not.
 """
 import functools
-import json
-import os
-import re
-import shutil
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
 import egate_oracle as ego
-import lsigf_oracle as orc
-import test_kernel_dispatch as kd
-from test_kernel_dispatch import F32, F64, NPD, SENT, Result, _check, _graph, _lib, _st
+from dispatch_harness import F32, F64, NPD, SENT, Result, _bits, _check, _graph, _lib, _st, check_case, child_traced
 
 MIXER = (0.6875, -1.3125)                  # 11/16, -21/16: exact products with grid values of s
 GRID = {"grid": (2.0 ** -10, 8.0), "large": (2.0 ** -4, 96.0)}
@@ -258,7 +252,7 @@ def _hop_case(dtype, N, Bs, C, ld, graph="rand", off=0, gate="bs", bwd="both", d
                 twin.append(("dsrc", fence("aligned dsrc", backward(0, src0)[0], 0)))
             for name, v in twin:
                 got = dict(outs)[name]
-                assert torch.equal(kd._bits(got), kd._bits(v)), "%s: misaligned and aligned runs differ" % name
+                assert torch.equal(_bits(got), _bits(v)), "%s: misaligned and aligned runs differ" % name
         return res
     return run
 
@@ -337,37 +331,6 @@ EGATE_CASES = [(cid, _attn_case(**kw), ks) for cid, kw, ks in ATTN_ROWS] + \
 
 
 # ------------------------------------------------------------------------------------------------------------ CPU
-def test_every_egate_kernel_has_a_case():
-    """Every __global__ function of egate.cu has a row here (they stay in test_kernel_dispatch.py's EXCLUDED, which
-    points at this file), and every name in this table is one of them."""
-    import test_nv_dispatch as nvd
-    found = {k for f, k in nvd._all_global_functions() if f == "egate.cu"}
-    assert len(found) == 5, sorted(found)
-    covered = nvd._covered(EGATE_CASES)
-    assert found == covered, (sorted(found), sorted(covered))
-    assert found <= set(kd.EXCLUDED) and all("test_egate_dispatch.py" in kd.EXCLUDED[k] for k in found)
-    ids = [c[0] for c in EGATE_CASES]
-    assert len(ids) == len(set(ids)) and not set(ids) & {c[0] for c in kd.CASES}
-
-
-def test_every_expected_egate_kernel_is_instantiated_in_the_library():
-    import gnn_b200
-    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    filt = shutil.which("cu++filt") or "/usr/local/cuda/bin/cu++filt"
-    if not (os.path.exists(tool) and os.path.exists(filt)):
-        pytest.skip("cuobjdump / cu++filt not available")
-    lib = gnn_b200._cabi.LIB_PATH
-    if not os.path.exists(lib):
-        pytest.skip("library not built")
-    syms = subprocess.run([tool, "-symbols", lib], capture_output=True, text=True, check=True).stdout
-    mangled = re.findall(r"STT_FUNC\s+.*?\s(\S+)\s*$", syms, flags=re.M)
-    names = [kd._norm(n) for n in subprocess.run([filt], input="\n".join(mangled), capture_output=True, text=True,
-                                                  check=True).stdout.splitlines()]
-    for cid, _, ks in EGATE_CASES:
-        for k in ks:
-            assert any(re.search(k, n) for n in names), (cid, k)
-
-
 def test_attention_rows_have_exact_zero_logits_and_underflow():
     """The grid rows contain logits that are exactly 0 (LeakyReLU'(0) = 0.2 on both sides), and the large-logit rows
     spread their logits over more than 100, enough to overflow an unshifted fp32 exp and underflow some alpha."""
@@ -383,72 +346,10 @@ def test_attention_rows_have_exact_zero_logits_and_underflow():
 
 
 # ------------------------------------------------------------------------------------------------------------ GPU
-def _profiled(fn, kernels, tries=4):
-    """The demangled names of the CUDA activities of one run of fn under torch.profiler.  A session can come back
-    without its GPU records (seen with torch 2.11 on an H100 once a process had been profiling for about two minutes:
-    alternate sessions empty, whatever they ran); fn is deterministic, so while some regex of `kernels` matches no
-    traced name the case is profiled again, up to `tries` times.  The caller still requires every expected kernel."""
-    from torch.profiler import ProfilerActivity, profile
-    for _ in range(tries):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        names = [kd._norm(e.name) for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-        if all(any(re.search(k, n) for n in names) for k in kernels):
-            break
-    return names
-
-
-def _trace_all(path):
-    """Writes {case id: traced names} of every row to path (JSON); run in a process of its own by `traced`."""
-    with open(path, "w") as f:
-        json.dump({cid: _profiled(fn, ks) for cid, fn, ks in EGATE_CASES}, f)
-
-
-@pytest.fixture(scope="module")
-def traced(tmp_path_factory):
-    """The kernels each row launches, traced in a fresh Python process.  The profiler degrades with the time since a
-    process first used it (see _profiled); tracing here would start that clock minutes before test_kernel_dispatch.py
-    and test_nv_dispatch.py profile their own rows later in the same pytest process.  A child process keeps this
-    table's sessions inside its own first minute and leaves the main process's profiler untouched."""
-    path = tmp_path_factory.mktemp("egate_trace") / "names.json"
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    env = dict(os.environ, PYTHONDONTWRITEBYTECODE="1",
-               PYTHONPATH=os.pathsep.join([here, os.path.join(root, "oracle"), root]
-                                          + [p for p in os.environ.get("PYTHONPATH", "").split(os.pathsep) if p]))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    subprocess.run([sys.executable] + flags + ["-c", "import sys, test_egate_dispatch as t; t._trace_all(sys.argv[1])",
-                                               str(path)], env=env, cwd=root, check=True, timeout=1800)
-    with open(path) as f:
-        return json.load(f)
+traced = child_traced("test_egate_dispatch", "EGATE_CASES")
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid,fn,kernels", EGATE_CASES, ids=[c[0] for c in EGATE_CASES])
 def test_egate_dispatch(cid, fn, kernels, traced):
-    names = traced[cid]
-    print("%s: %s" % (cid, sorted(set(n.split("(")[0] for n in names if "kernel" in n))))
-    remaining = list(names)
-    for k in kernels:   # a regex listed twice must match two launches
-        hit = next((n for n in remaining if re.search(k, n)), None)
-        assert hit is not None, "%s: expected %s among %s" % (cid, k, sorted(set(n.split("(")[0] for n in names)))
-        remaining.remove(hit)
-    res1 = fn()
-    torch.cuda.synchronize()
-    worst = []
-    for name, out, ref, bound in res1.checks:
-        v = orc.bound_violation(out.detach().double().cpu().numpy(), ref, bound)
-        worst.append("%s %.3g" % (name, v))
-        assert v <= 1.0, "%s/%s: error %.3g x its bound" % (cid, name, v)
-    print("%s: worst error / bound: %s" % (cid, ", ".join(worst)))
-    for name, t in res1.canaries:
-        assert torch.equal(kd._bits(t), kd._bits(torch.full_like(t, SENT))), "%s: wrote outside its contract (%s)" % (
-            cid, name)
-    for name, t in res1.finite:
-        assert bool(torch.isfinite(t).all()), "%s: non-finite %s (NaN in an input pad leaked)" % (cid, name)
-    res2 = fn()
-    torch.cuda.synchronize()
-    for a, b in zip(res1.outputs, res2.outputs):
-        assert torch.equal(kd._bits(a), kd._bits(b)), "%s: two runs differ" % cid
+    check_case(cid, fn, kernels, traced[cid])

@@ -17,7 +17,7 @@ import torch
 import egate_oracle as ego
 import lsigf_oracle as orc
 import test_egate_dispatch as ed
-from test_kernel_dispatch import F32, NPD
+from dispatch_harness import F32, NPD
 
 WIDE = 3.0
 MIXER = ed.MIXER

@@ -2,22 +2,15 @@
 
 Every row of CASES names an entry point, the shape / layout / alignment that selects a branch, and the kernels that
 branch must launch (regexes on the demangled name, template arguments included).  The GPU test runs the case once under
-torch.profiler, asserts those kernels ran, then checks every output against oracle/lsigf_oracle.py's componentwise bound
-(oracle/ev_oracle.py's for the edge-variant filter), checks that memory outside the kernel's contract kept its canary
-pattern, and that a second run is bit-identical.
-The CPU tests keep the table honest: every __global__ function in csrc/ is covered by a case or excluded with a reason,
-and every regex matches a kernel instantiated in the built library.
+torch.profiler in the pytest process and holds it to tests/dispatch_harness.py's check_case: those kernels ran, every
+output is within oracle/lsigf_oracle.py's componentwise bound (oracle/ev_oracle.py's for the edge-variant filter),
+memory outside the kernel's contract kept its canary pattern, and a second run is bit-identical.  This table owns the
+kernels of csrc/*.cu and csrc/*.cuh except egate.cu: tests/test_dispatch_tables.py requires each of them to have a
+case here or an entry in EXCLUDED.
 
 Determinism exemption: maxpool_backward scatters with atomicAdd, so the order of its additions (and its last bits) may
 change from run to run; its case checks only the bound.
 """
-import functools
-import glob
-import os
-import re
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 import scipy.sparse as sp
@@ -25,76 +18,11 @@ import torch
 
 import ev_oracle as evo
 import lsigf_oracle as orc
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "graph-neural-networks_b200", "csrc")
-SENT = -7.125e30            # canary value: exactly representable in fp32 and fp64, never produced by these inputs
-F32, F64 = torch.float32, torch.float64
-NPD = {F32: np.float32, F64: np.float64}
-
-
-def _lib():
-    import gnn_b200
-    return gnn_b200._cabi, gnn_b200._cabi.load()
-
-
-def _st():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _check(rc):
-    cabi, lib = _lib()
-    assert rc == 0, lib.b200gf_strerror(rc)
-
-
-def _padded(C, dtype):
-    q = 32 // torch.empty(0, dtype=dtype).element_size()
-    return (C + q - 1) // q * q
-
-
-class Result:
-    """What a case run hands back: outputs (tensors, compared bit-for-bit across runs), checks (name, out, ref, bound),
-    canaries (name, tensor that must equal SENT bit-for-bit) and finite (name, tensor that must be all finite)."""
-
-    def __init__(self):
-        self.outputs, self.checks, self.canaries, self.finite = [], [], [], []
+from dispatch_harness import (F32, F64, NPD, SENT, Result, _bits, _check, _from_node_major, _graph, _launched, _lib,
+                              _padded, _st, check_case)
 
 
 # ---------------------------------------------------------------------------------------------------------------- hop
-@functools.lru_cache(maxsize=None)
-def _graph(kind, N, seed=0):
-    """Row lengths 0, 1, S*U-1 .. S*U+1 of every lane mapping (S*U = 4, 8, 16, 32), 31..65, 127..129, a self-loop, a
-    neighbour in column N-1, and (N > 20000) a hub row of 20 000 entries; the transpose gets the same lengths through
-    the long columns added at the end."""
-    rng = np.random.default_rng(seed + N)
-    special = [0, 1, 3, 4, 5, 7, 8, 9, 15, 16, 17, 31, 32, 33, 63, 64, 65, 127, 128, 129]
-    if kind == "tiny":
-        special = special[:N]
-    lens = list(rng.integers(0, 9, N))
-    for i, L in enumerate(special[:N]):
-        lens[i] = min(L, N)
-    if N > 20000:
-        lens[N // 2] = 20000
-    rows, cols = [], []
-    for r, L in enumerate(lens):
-        rows += [r] * int(L)
-        cols += list(rng.choice(N, size=int(L), replace=False))
-    # long columns (rows of S^T) of the same lengths, in columns N-1, N-2, ...
-    for i, L in enumerate(special[:N] + ([20000] if N > 20000 else [])):
-        if N >= 60:
-            rows += list(rng.choice(N, size=min(L, N), replace=False))
-            cols += [N - 1 - i] * min(L, N)
-    rows += [min(3, N - 1), min(5, N - 1)]
-    cols += [min(3, N - 1), N - 1]                       # self-loop, neighbour N-1
-    m = sp.coo_matrix((rng.standard_normal(len(rows)), (rows, cols)), shape=(N, N)).tocsr()
-    m.sum_duplicates()
-    if kind == "sym":
-        m = sp.triu(m, 1) + sp.triu(m, 1).T + sp.diags(m.diagonal())
-        m = sp.csr_matrix(m)
-    m.sort_indices()
-    return m
-
-
 def _hop_case(dtype, C, ld, N=3000, graph="rand", src_off=0, dst_off=0, plan_kind="full"):
     """b200gf_hop, both directions: src [n_cols, ld] with NaN in its pad columns, dst [n_rows + 3, ld] of SENT."""
     def run():
@@ -482,10 +410,6 @@ def _node_major(t_bfn, ld):
     return out
 
 
-def _from_node_major(t, B, C, N):
-    return t[:N, :B * C].reshape(N, B, C).permute(1, 2, 0)
-
-
 def _lsigf_autograd_case(dtype, N, B, G, F, K, E, bias="F1"):
     """gnn_b200.LSIGF forward + autograd backward against the sparse oracle and its envelope."""
     def run():
@@ -791,113 +715,18 @@ def _ev_rows():
 CASES = (_hop_rows() + _contract_rows() + _tap_grad_rows() + _bias_grad_rows() + _lsigf_rows() + _layout_rows()
          + _layer_rows() + _ev_rows())
 
-# __global__ functions without a case here, and where they are tested
-EGATE = "edge-gated layer: tests/test_egate_dispatch.py keeps its own case table, one row per egate.cu launch branch"
+# __global__ functions of this table's sources without a case here, and where they are tested
 EXCLUDED = {
     "peer_signal_kernel": "multi-process peer fence: tests/test_distributed.py",
     "peer_wait_kernel": "multi-process peer fence: tests/test_distributed.py",
     "bcast_rows_kernel": "all-gather epilogue of the node-sharded path: tests/test_cabi.py, tests/test_distributed.py",
     "scatter_rows_kernel": "scatter epilogue of the feature-sharded path: tests/test_cabi.py, tests/test_distributed.py",
     "narrow_rowptr_kernel": "device plan build (b200gf_plan_create_device): tests/test_widen_*",
-    "egate_softmax_kernel": EGATE,
-    "egate_softmax_bwd_kernel": EGATE,
-    "egate_colsum_kernel": EGATE,
-    "egate_hop_kernel": EGATE,
-    "egate_sddmm_kernel": EGATE,
 }
-
-
-def _norm(name):
-    """Demangled kernel name without casts and spaces: 'spmm_hop_kernel<float, (int)4, ...' -> 'spmm_hop_kernel<float,4,...'."""
-    name = re.sub(r"\((?:int|bool|unsigned int|long)\)", "", name)
-    return name.replace(" ", "").replace("true", "1").replace("false", "0")
-
-
-# ------------------------------------------------------------------------------------------------------------ CPU
-def _global_functions():
-    names = set()
-    for path in glob.glob(os.path.join(CSRC, "*.cu")) + glob.glob(os.path.join(CSRC, "*.cuh")):
-        src = open(path).read()
-        # __launch_bounds__ may come before or after the return type
-        names.update(re.findall(r"__global__\s+(?:__launch_bounds__\([^)]*\)\s*)?void\s+(?:__launch_bounds__\([^)]*\)\s*)?"
-                                r"(\w+)\s*\(", src))
-    return names
-
-
-def test_every_global_function_has_a_case_or_an_exclusion():
-    names = _global_functions()
-    assert len(names) >= 36, sorted(names)
-    covered = {re.match(r"\w+", k).group(0) for _, _, ks in CASES for k in ks}
-    missing = sorted(n for n in names if n not in covered and n not in EXCLUDED)
-    assert not missing, "kernels without a dispatch case or an exclusion: %s" % missing
-    stale = sorted(set(EXCLUDED) - names) + sorted(covered - names)
-    assert not stale, "table names that are not __global__ functions in csrc/: %s" % stale
-    ids = [c[0] for c in CASES]
-    assert len(ids) == len(set(ids))
-
-
-def test_every_expected_kernel_is_instantiated_in_the_library():
-    """Each regex of the table matches a kernel compiled into libb200gf.so (so a typo fails here, not on the GPU)."""
-    import gnn_b200
-    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    filt = shutil.which("cu++filt") or "/usr/local/cuda/bin/cu++filt"
-    if not (os.path.exists(tool) and os.path.exists(filt)):
-        pytest.skip("cuobjdump / cu++filt not available")
-    lib = gnn_b200._cabi.LIB_PATH
-    if not os.path.exists(lib):
-        pytest.skip("library not built")
-    syms = subprocess.run([tool, "-symbols", lib], capture_output=True, text=True, check=True).stdout
-    mangled = re.findall(r"STT_FUNC\s+.*?\s(\S+)\s*$", syms, flags=re.M)
-    names = [_norm(n) for n in subprocess.run([filt], input="\n".join(mangled), capture_output=True, text=True,
-                                               check=True).stdout.splitlines()]
-    for cid, _, ks in CASES:
-        for k in ks:
-            assert any(re.search(k, n) for n in names), (cid, k)
-
-
-# ------------------------------------------------------------------------------------------------------------ GPU
-def _launched(fn):
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        res = fn()
-        torch.cuda.synchronize()
-    names = [_norm(e.name) for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-    return res, names
-
-
-def _bits(t):
-    t = t.detach().contiguous()
-    return t.view(torch.int32 if t.element_size() == 4 else torch.int64) if t.is_floating_point() else t
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid,fn,kernels", CASES, ids=[c[0] for c in CASES])
 def test_dispatch(cid, fn, kernels):
     res1, names = _launched(fn)
-    kern = [n for n in names if "kernel" in n]
-    print("%s: %s" % (cid, sorted(set(n.split("(")[0] for n in kern))))
-    remaining = list(names)
-    for k in kernels:   # a regex listed twice must match two launches
-        hit = next((n for n in remaining if re.search(k, n)), None)
-        assert hit is not None, "%s: expected %s among %s" % (cid, k, sorted(set(n.split("(")[0] for n in names)))
-        remaining.remove(hit)
-    worst = []
-    for name, out, ref, bound in res1.checks:
-        if ref is None:
-            continue
-        v = orc.bound_violation(out.detach().double().cpu().numpy(), ref, bound)
-        worst.append("%s %.3g" % (name, v))
-        assert v <= 1.0, "%s/%s: error %.3g x its bound" % (cid, name, v)
-    print("%s: worst error / bound: %s" % (cid, ", ".join(worst) or "exact"))
-    for name, t in res1.canaries:
-        assert torch.equal(_bits(t), _bits(torch.full_like(t, SENT if t.is_floating_point() else 0x5A))), \
-            "%s: wrote outside its contract (%s)" % (cid, name)
-    for name, t in res1.finite:
-        assert bool(torch.isfinite(t).all()), "%s: non-finite %s (NaN in an input pad leaked)" % (cid, name)
-    if getattr(res1, "nondeterministic", False):
-        return
-    res2 = fn()
-    torch.cuda.synchronize()
-    for a, b in zip(res1.outputs, res2.outputs):
-        assert torch.equal(_bits(a), _bits(b)), "%s: two runs differ" % cid
+    check_case(cid, fn, kernels, names, res1)

@@ -1,29 +1,20 @@
 """One case per dispatch branch of the node-variant filter's kernels (csrc/nv/nv.cu), each held to oracle/nv_oracle.py's
-componentwise fp64 bound, in the format of tests/test_kernel_dispatch.py and with its helpers.
+componentwise fp64 bound.
 
 Every row names the kernels its branch must launch (regexes on the demangled name).  The GPU test runs the case once under
-torch.profiler, asserts those kernels ran, checks every output against its bound, checks that memory outside the kernels'
-contract kept its canary pattern, that NaN in input pad columns reached no output, and that a second run is bit-identical.
-The CPU tests keep the tables honest: every __global__ function anywhere under csrc/ (subdirectories included) has a case
-in this table or in test_kernel_dispatch.py's (or is excluded there), and every regex here matches a kernel compiled into
-the library.
+torch.profiler in the pytest process and holds it to tests/dispatch_harness.py's check_case: those kernels ran, every
+output is within its bound, memory outside the kernels' contract kept its canary pattern, NaN in input pad columns
+reached no output, and a second run is bit-identical.  This table owns the kernels of csrc/nv/
+(tests/test_dispatch_tables.py).
 """
-import glob
-import os
-import re
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 import scipy.sparse as sp
 import torch
 
 import lsigf_oracle as orc
-import test_kernel_dispatch as kd
-from test_kernel_dispatch import F32, F64, NPD, SENT, Result, _check, _from_node_major, _graph, _lib, _st
-
-CSRC = kd.CSRC
+from dispatch_harness import (F32, F64, NPD, SENT, Result, _check, _from_node_major, _graph, _launched, _lib, _st,
+                              check_case)
 
 
 def _nv_case(dtype, N, B, G, F, K, E, M, bias="F1", graph="rand", x_pad=3):
@@ -142,81 +133,9 @@ def _nv_rows():
 NV_CASES = _nv_rows()
 
 
-# ------------------------------------------------------------------------------------------------------------ CPU
-def _all_global_functions():
-    """(file, kernel) for every __global__ function in csrc/ and its subdirectories."""
-    out = set()
-    for path in glob.glob(os.path.join(CSRC, "**", "*.cu"), recursive=True) + \
-            glob.glob(os.path.join(CSRC, "**", "*.cuh"), recursive=True):
-        src = open(path).read()
-        for name in re.findall(r"__global__\s+(?:__launch_bounds__\([^)]*\)\s*)?void\s+"
-                               r"(?:__launch_bounds__\([^)]*\)\s*)?(\w+)\s*\(", src):
-            out.add((os.path.relpath(path, CSRC), name))
-    return out
-
-
-def _covered(cases):
-    return {re.match(r"\w+", k).group(0) for _, _, ks in cases for k in ks}
-
-
-def test_every_global_function_in_csrc_has_a_case():
-    """No kernel anywhere under csrc/ goes without a dispatch case: the node-variant kernels need one here, every other
-    kernel one in test_kernel_dispatch.py (or its listed exclusion)."""
-    found = _all_global_functions()
-    nv = {k for f, k in found if f.startswith("nv" + os.sep)}
-    assert nv, "no kernels found under csrc/nv/"
-    missing_nv = sorted(nv - _covered(NV_CASES))
-    assert not missing_nv, "node-variant kernels without a dispatch case: %s" % missing_nv
-    others = {k for f, k in found if not f.startswith("nv" + os.sep)}
-    missing = sorted(others - _covered(kd.CASES) - set(kd.EXCLUDED))
-    assert not missing, "kernels without a dispatch case or an exclusion: %s" % missing
-    stale = sorted(_covered(NV_CASES) - nv)
-    assert not stale, "table names that are not __global__ functions in csrc/nv/: %s" % stale
-    ids = [c[0] for c in NV_CASES]
-    assert len(ids) == len(set(ids)) and not set(ids) & {c[0] for c in kd.CASES}
-
-
-def test_every_expected_nv_kernel_is_instantiated_in_the_library():
-    import gnn_b200
-    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    filt = shutil.which("cu++filt") or "/usr/local/cuda/bin/cu++filt"
-    if not (os.path.exists(tool) and os.path.exists(filt)):
-        pytest.skip("cuobjdump / cu++filt not available")
-    lib = gnn_b200._cabi.LIB_PATH
-    if not os.path.exists(lib):
-        pytest.skip("library not built")
-    syms = subprocess.run([tool, "-symbols", lib], capture_output=True, text=True, check=True).stdout
-    mangled = re.findall(r"STT_FUNC\s+.*?\s(\S+)\s*$", syms, flags=re.M)
-    names = [kd._norm(n) for n in subprocess.run([filt], input="\n".join(mangled), capture_output=True, text=True,
-                                                  check=True).stdout.splitlines()]
-    for cid, _, ks in NV_CASES:
-        for k in ks:
-            assert any(re.search(k, n) for n in names), (cid, k)
-
-
 # ------------------------------------------------------------------------------------------------------------ GPU
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid,fn,kernels", NV_CASES, ids=[c[0] for c in NV_CASES])
 def test_nv_dispatch(cid, fn, kernels):
-    res1, names = kd._launched(fn)
-    print("%s: %s" % (cid, sorted(set(n.split("(")[0] for n in names if "kernel" in n))))
-    remaining = list(names)
-    for k in kernels:   # a regex listed twice must match two launches
-        hit = next((n for n in remaining if re.search(k, n)), None)
-        assert hit is not None, "%s: expected %s among %s" % (cid, k, sorted(set(n.split("(")[0] for n in names)))
-        remaining.remove(hit)
-    worst = []
-    for name, out, ref, bound in res1.checks:
-        v = orc.bound_violation(out.detach().double().cpu().numpy(), ref, bound)
-        worst.append("%s %.3g" % (name, v))
-        assert v <= 1.0, "%s/%s: error %.3g x its bound" % (cid, name, v)
-    print("%s: worst error / bound: %s" % (cid, ", ".join(worst)))
-    for name, t in res1.canaries:
-        assert torch.equal(kd._bits(t), kd._bits(torch.full_like(t, SENT if t.is_floating_point() else 0x5A))), \
-            "%s: wrote outside its contract (%s)" % (cid, name)
-    for name, t in res1.finite:
-        assert bool(torch.isfinite(t).all()), "%s: non-finite %s (NaN in an input pad leaked)" % (cid, name)
-    res2 = fn()
-    torch.cuda.synchronize()
-    for a, b in zip(res1.outputs, res2.outputs):
-        assert torch.equal(kd._bits(a), kd._bits(b)), "%s: two runs differ" % cid
+    res1, names = _launched(fn)
+    check_case(cid, fn, kernels, names, res1)

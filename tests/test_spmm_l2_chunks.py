@@ -10,22 +10,13 @@ a rerun must be bit-identical.  Partitioned plans ignore the override.  When not
 taken for rows of at most 256 bytes of a graph whose gathers spread over the whole source if a chunk is at most 3x the
 L2; a banded graph and wider rows keep the row width's chunk.
 """
-import json
-import os
-import re
-import shutil
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import scipy.sparse as sp
 import torch
 
 import lsigf_oracle as orc
-import test_kernel_dispatch as kd
-from test_egate_dispatch import _profiled
-from test_kernel_dispatch import F32, F64, NPD, SENT, Result, _check, _graph, _lib, _padded, _st
+from dispatch_harness import F32, F64, NPD, SENT, Result, _check, _graph, _lib, _padded, _st, check_case, child_traced
 
 
 def _band(N, half=20, seed=0):
@@ -170,79 +161,16 @@ def _rows():
 CASES = _rows()
 
 
-def test_case_ids_are_unique_and_new():
-    ids = [c[0] for c in CASES]
-    assert len(ids) == len(set(ids)) and not set(ids) & {c[0] for c in kd.CASES}
-
-
-def test_every_expected_kernel_is_instantiated_in_the_library():
-    import gnn_b200
-    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    filt = shutil.which("cu++filt") or "/usr/local/cuda/bin/cu++filt"
-    if not (os.path.exists(tool) and os.path.exists(filt)):
-        pytest.skip("cuobjdump / cu++filt not available")
-    lib = gnn_b200._cabi.LIB_PATH
-    if not os.path.exists(lib):
-        pytest.skip("library not built")
-    syms = subprocess.run([tool, "-symbols", lib], capture_output=True, text=True, check=True).stdout
-    mangled = re.findall(r"STT_FUNC\s+.*?\s(\S+)\s*$", syms, flags=re.M)
-    names = [kd._norm(n) for n in subprocess.run([filt], input="\n".join(mangled), capture_output=True, text=True,
-                                                  check=True).stdout.splitlines()]
-    for cid, _, ks in CASES:
-        for k in ks:
-            assert any(re.search(k, n) for n in names), (cid, k)
-
-
 def test_set_l2_bytes_rejects_bad_arguments_without_gpu():
     cabi, lib = _lib()
     assert lib.b200gf_plan_set_l2_bytes(None, 0) == -1
     assert lib.b200gf_plan_info(None, 7) == -1
 
 
-def _trace_all(path):
-    """Writes {case id: traced names} of every row to path (JSON); run in a process of its own by `traced`."""
-    with open(path, "w") as f:
-        json.dump({cid: _profiled(fn, ks) for cid, fn, ks in CASES}, f)
-
-
-@pytest.fixture(scope="module")
-def traced(tmp_path_factory):
-    """The kernels each row launches, traced in a fresh Python process, as tests/test_egate_dispatch.py does: profiling
-    sessions in a long-running process can come back without their GPU records, and tracing here would start that clock
-    while other test files profile in the pytest process."""
-    path = tmp_path_factory.mktemp("l2_chunk_trace") / "names.json"
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    env = dict(os.environ, PYTHONDONTWRITEBYTECODE="1",
-               PYTHONPATH=os.pathsep.join([here, os.path.join(root, "oracle"), root]
-                                          + [p for p in os.environ.get("PYTHONPATH", "").split(os.pathsep) if p]))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    subprocess.run([sys.executable] + flags + ["-c", "import sys, test_spmm_l2_chunks as t; t._trace_all(sys.argv[1])",
-                                               str(path)], env=env, cwd=root, check=True, timeout=1800)
-    with open(path) as f:
-        return json.load(f)
+traced = child_traced("test_spmm_l2_chunks", "CASES")
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid,fn,kernels", CASES, ids=[c[0] for c in CASES])
 def test_chunk(cid, fn, kernels, traced):
-    names = traced[cid]
-    for k in kernels:
-        assert any(re.search(k, n) for n in names), "%s: expected %s among %s" % (
-            cid, k, sorted(set(n.split("(")[0] for n in names if "kernel" in n)))
-    res1 = fn()
-    torch.cuda.synchronize()
-    worst = []
-    for name, out, ref, bound in res1.checks:
-        v = orc.bound_violation(out.detach().double().cpu().numpy(), ref, bound)
-        worst.append("%s %.3g" % (name, v))
-        assert v <= 1.0, "%s/%s: error %.3g x its bound" % (cid, name, v)
-    print("%s: worst error / bound: %s" % (cid, ", ".join(worst) or "oracle tolerance"))
-    for name, t in res1.canaries:
-        assert torch.equal(kd._bits(t), kd._bits(torch.full_like(t, SENT))), "%s: wrote outside its contract (%s)" % (cid, name)
-    for name, t in res1.finite:
-        assert bool(torch.isfinite(t).all()), "%s: non-finite %s (NaN in an input pad leaked)" % (cid, name)
-    res2 = fn()
-    torch.cuda.synchronize()
-    for a, b in zip(res1.outputs, res2.outputs):
-        assert torch.equal(kd._bits(a), kd._bits(b)), "%s: two runs differ" % cid
+    check_case(cid, fn, kernels, traced[cid])

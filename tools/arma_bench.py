@@ -2,7 +2,7 @@
 """ARMA filter (gnn_b200.jARMA) timings on an Erdos-Renyi graph, with CUDA events.
 
 Prints the card and its power limit, then for a zero-diagonal GSO (the constant-diagonal path: an LSIGF over S~^T with
-tMax + 2 taps) and a combinatorial Laplacian L = D - A (a varying diagonal: the general path, csrc_arma/arma.cu):
+tMax + 2 taps) and a combinatorial Laplacian L = D - A (a varying diagonal: the general path, csrc/arma/arma.cu):
 forward and forward + backward ms; for the general path the wide hop's time, its gather-model bytes
 nnz (4 + s) + (N + 1) 8 + nnz C s + N C s (C = 2 B F P G) and the rate they imply, and the share of the step spent in
 arma.cu's element-wise kernels (torch.profiler, a run of its own); GraphFilter at the same G, F and K as a yardstick;

@@ -2,7 +2,8 @@
 """nvcc -Xptxas -v output (stdin or file) -> one line per kernel: registers, stack, spill stores/loads, smem.
    usage: nvcc ... -Xptxas -v ... 2>&1 | python tools/ptxas_report.py [filter-substring]
    The library's sources are graph-neural-networks_b200/build.py's SOURCES: csrc/*.cu, csrc/nv/nv.cu and
-   csrc_arma/arma.cu (e.g. `... -c graph-neural-networks_b200/csrc_arma/arma.cu ... | python tools/ptxas_report.py arma_`)."""
+   csrc/arma/arma.cu
+   (e.g. `... -c graph-neural-networks_b200/csrc/arma/arma.cu ... | python tools/ptxas_report.py arma_`)."""
 import re
 import subprocess
 import sys
@@ -33,7 +34,7 @@ try:
 except Exception:
     dem = names
 for r, d in zip(rows, dem):
-    # kernels in an anonymous namespace (csrc/nv/nv.cu, csrc_arma/arma.cu) demangle with "(anonymous namespace)::"
+    # kernels in an anonymous namespace (csrc/nv/nv.cu, csrc/arma/arma.cu) demangle with "(anonymous namespace)::"
     d = re.sub(r"\(.*", "", d.replace("(anonymous namespace)::", "")).replace("void b200gf::", "").replace("void ", "")
     if flt and flt not in d:
         continue
