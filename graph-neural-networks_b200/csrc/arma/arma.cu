@@ -21,21 +21,14 @@
 // over (i, b) by a deterministic two-pass column sum over fixed row pieces.
 #include "../common.cuh"
 
-#include <algorithm>
-
 using namespace b200gf;
 
 namespace {
 
 constexpr int ARMA_THREADS = 256;
-constexpr int ARMA_PIECES_TARGET = 1024;       // the column sums cut N rows into about this many pieces
 
-int64_t arma_chunk(int64_t N) { return std::max<int64_t>(32, (N + ARMA_PIECES_TARGET - 1) / ARMA_PIECES_TARGET); }
-int64_t arma_pieces(int64_t N) { return N == 0 ? 0 : (N + arma_chunk(N) - 1) / arma_chunk(N); }
-
-int grid_for(int64_t total, int threads, int sm_count) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((total + threads - 1) / threads, (int64_t)sm_count * 8));
-}
+// the column sums cut N rows into pieces of piece_rows(N) rows
+int64_t arma_pieces(int64_t N) { return N == 0 ? 0 : (N + piece_rows(N) - 1) / piece_rows(N); }
 
 // ---------------------------------------------------------------------------------------------------------------
 // forward: one thread per output (i, b, f), over the P G contiguous columns of (b, f) in both chains.
@@ -178,17 +171,6 @@ arma_colsum_reduce_kernel(int64_t pieces, int F, int P, int G, int E, int e, con
   }
 }
 
-struct Carver {
-  char* base;
-  size_t off = 0;
-  explicit Carver(void* p) : base((char*)p) {}
-  void* take(size_t bytes) {
-    void* r = base ? base + off : nullptr;
-    off += align_up(bytes, 256);
-    return r;
-  }
-};
-
 struct ArmaDims {
   int64_t N, C, Q, ldw, ldn;
   size_t es, wide, narrow;
@@ -252,7 +234,7 @@ int launch_scale_acc(bool seed, const b200gf_plan* p, int B, int G, int F, int P
                      const void* varphi, const void* x, int64_t x_ld, const void* sx, int64_t sx_ld, void* state,
                      int64_t ldw, int t, int tMax, void* out, int64_t out_ld, cudaStream_t st) {
   const int64_t N = p->n_rows;
-  const int grid = grid_for(N * B * F, ARMA_THREADS, p->sm_count);
+  const int grid = grid_for(N * B * F, ARMA_THREADS, p->sm_count * 8);
   const T sgn = (t & 1) ? T(-1) : T(1), h2 = ((tMax + 1) & 1) ? T(-1) : T(1);
   const T* dd = (const T*)d + (int64_t)e * N;
   if (seed)
@@ -300,10 +282,10 @@ int arma_backward_t(const b200gf_plan* p, const void* d, const void* psi, const 
   const int64_t N = a.N;
   const int E = p->E;
   const int sms = p->sm_count;
-  const int gstep = grid_for(N * B * F, ARMA_THREADS, sms);
-  const int gfold = grid_for(N * B * G, ARMA_THREADS, sms);
+  const int gstep = grid_for(N * B * F, ARMA_THREADS, sms * 8);
+  const int gfold = grid_for(N * B * G, ARMA_THREADS, sms * 8);
   const T h2 = ((tMax + 1) & 1) ? T(-1) : T(1);
-  const int64_t chunk = arma_chunk(N), pieces = arma_pieces(N);
+  const int64_t chunk = piece_rows(N), pieces = arma_pieces(N);
   int rc;
   for (int e = 0; e < E; ++e) {
     const T* dd = (const T*)d + (int64_t)e * N;
@@ -332,7 +314,7 @@ int arma_backward_t(const b200gf_plan* p, const void* d, const void* psi, const 
     }
     arma_colsum_partial_kernel<T><<<(unsigned)pieces, ARMA_THREADS, 0, st>>>(N, B, a.Q, (const T*)w.acc, a.ldw, chunk,
                                                                             (T*)w.partial);
-    arma_colsum_reduce_kernel<T><<<grid_for(2 * a.Q, ARMA_THREADS, sms), ARMA_THREADS, 0, st>>>(
+    arma_colsum_reduce_kernel<T><<<grid_for(2 * a.Q, ARMA_THREADS, sms * 8), ARMA_THREADS, 0, st>>>(
         pieces, F, P, G, E, e, (const T*)w.partial, (T*)dpsi, (T*)dvarphi);
     LAUNCH_CHECK_N(2);
   }
@@ -355,15 +337,15 @@ int b200gf_arma_forward(const b200gf_plan* plan, const void* d, const void* psi,
   if (arma_bad_dims(plan, tMax, B, G, F, P) || !d || !psi || !varphi || !x || !out) return B200GF_EINVAL;
   if (x_ld < (int64_t)B * G || out_ld < (int64_t)B * F) return B200GF_EINVAL;
   if (arma_too_wide(B, G, F, P)) return B200GF_EUNSUPPORTED;
-  if (!workspace || ((uintptr_t)workspace & 255) != 0) return workspace ? B200GF_EINVAL : B200GF_EWORKSPACE;
-  if (states && ((uintptr_t)states & 255) != 0) return B200GF_EINVAL;
+  // a misaligned states buffer is reported after a missing workspace and before a short one
+  if (workspace && states && ((uintptr_t)states & 255) != 0) return B200GF_EINVAL;
   const ArmaWs w = carve_arma(plan, workspace, B, G, F, P, states ? 1 : 0);
-  if (w.bytes > workspace_bytes) return B200GF_EWORKSPACE;
+  if (int rc = check_workspace(workspace, w.bytes, workspace_bytes, true)) return rc;
   if (plan->n_rows == 0) return B200GF_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (plan->dtype == B200GF_F32)
-    return arma_forward_t<float>(plan, d, psi, varphi, tMax, B, G, F, P, x, x_ld, out, out_ld, states, w, st);
-  return arma_forward_t<double>(plan, d, psi, varphi, tMax, B, G, F, P, x, x_ld, out, out_ld, states, w, st);
+  return with_dtype(plan->dtype, [&](auto tag) {
+    return arma_forward_t<decltype(tag)>(plan, d, psi, varphi, tMax, B, G, F, P, x, x_ld, out, out_ld, states, w,
+                                         (cudaStream_t)stream);
+  });
 }
 
 int b200gf_arma_backward(const b200gf_plan* plan, const void* d, const void* psi, const void* varphi, int tMax, int B,
@@ -373,9 +355,8 @@ int b200gf_arma_backward(const b200gf_plan* plan, const void* d, const void* psi
   if (!d || !psi || !varphi || !dy || !states || !dpsi || !dvarphi) return B200GF_EINVAL;
   if (dy_ld < (int64_t)B * F || (dx && dx_ld < (int64_t)B * G)) return B200GF_EINVAL;
   if (arma_too_wide(B, G, F, P)) return B200GF_EUNSUPPORTED;
-  if (!workspace || ((uintptr_t)workspace & 255) != 0) return workspace ? B200GF_EINVAL : B200GF_EWORKSPACE;
   const ArmaWs w = carve_arma(plan, workspace, B, G, F, P, 2);
-  if (w.bytes > workspace_bytes) return B200GF_EWORKSPACE;
+  if (int rc = check_workspace(workspace, w.bytes, workspace_bytes, true)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (plan->n_rows == 0) {
     const size_t n = (size_t)F * plan->E * P * G * dtype_size(plan->dtype);
@@ -383,11 +364,10 @@ int b200gf_arma_backward(const b200gf_plan* plan, const void* d, const void* psi
     CUDA_TRY(cudaMemsetAsync(dvarphi, 0, n, st));
     return B200GF_OK;
   }
-  if (plan->dtype == B200GF_F32)
-    return arma_backward_t<float>(plan, d, psi, varphi, tMax, B, G, F, P, dy, dy_ld, states, dx, dx_ld, dpsi, dvarphi,
-                                  w, st);
-  return arma_backward_t<double>(plan, d, psi, varphi, tMax, B, G, F, P, dy, dy_ld, states, dx, dx_ld, dpsi, dvarphi, w,
-                                 st);
+  return with_dtype(plan->dtype, [&](auto tag) {
+    return arma_backward_t<decltype(tag)>(plan, d, psi, varphi, tMax, B, G, F, P, dy, dy_ld, states, dx, dx_ld, dpsi,
+                                          dvarphi, w, st);
+  });
 }
 
 }  // extern "C"

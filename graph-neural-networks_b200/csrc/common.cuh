@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
+#include <algorithm>
 #include <atomic>
 #include <type_traits>
 #include <vector>
@@ -52,6 +53,42 @@ inline int64_t padded_ld(int64_t C, int dtype) {
   return (C + q - 1) / q * q;
 }
 
+// f(float{}) or f(double{}) for the dtype, B200GF_EUNSUPPORTED for any other; f names its type as decltype(tag)
+template <typename Fn>
+int with_dtype(int dtype, Fn&& f) {
+  if (dtype == B200GF_F32) return f(float{});
+  if (dtype == B200GF_F64) return f(double{});
+  return B200GF_EUNSUPPORTED;
+}
+
+// blocks of `threads` for a grid-stride loop over `total` items: one item per thread, at most `cap` blocks, at least one
+inline int grid_for(int64_t total, int threads, int64_t cap) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((total + threads - 1) / threads, cap));
+}
+
+// rows per piece of the deterministic two-pass sums: about 1024 pieces, at least 32 rows each
+inline int64_t piece_rows(int64_t N) { return std::max<int64_t>(32, (N + 1023) / 1024); }
+
+// consecutive 256-byte aligned slices of the caller's workspace; with a null base it only adds up the bytes (off)
+struct Carver {
+  char* base;
+  size_t off = 0;
+  explicit Carver(void* p) : base((char*)p) {}
+  void* take(size_t bytes) {
+    void* r = base ? base + off : nullptr;
+    off += align_up(bytes, 256);
+    return r;
+  }
+};
+
+// the caller's workspace: EINVAL when not 256-byte aligned, EWORKSPACE when null although `required` or `need` > 0,
+// EWORKSPACE when smaller than `need`
+inline int check_workspace(const void* ws, size_t need, size_t have, bool required) {
+  if (ws && ((uintptr_t)ws & 255) != 0) return B200GF_EINVAL;
+  if (!ws && (required || need > 0)) return B200GF_EWORKSPACE;
+  return need > have ? B200GF_EWORKSPACE : B200GF_OK;
+}
+
 // type-erased description of the fused NVLink scatter epilogue (spmm_kernels.cuh: ScatterArgs)
 struct ScatterHost {
   void* peer[16];
@@ -82,6 +119,16 @@ struct TermList {            // passed by value to kernels: up to MAX_TERMS (poi
   const void* ptr[MAX_TERMS];
   int64_t ld[MAX_TERMS];
 };
+
+// the first n terms of the arrays zs / z_ld (n <= MAX_TERMS)
+inline TermList make_terms(const void* const* zs, const int64_t* z_ld, int n) {
+  TermList tl;
+  for (int i = 0; i < n; ++i) {
+    tl.ptr[i] = zs[i];
+    tl.ld[i] = z_ld[i];
+  }
+  return tl;
+}
 
 int launch_tap_contract(int dtype, int64_t n_rows, int B, int P, int Q, int T, const void* const* zs,
                         const int64_t* z_ld, const void* W, const void* bias, int bias_per_node,
@@ -143,4 +190,9 @@ namespace b200gf {
 // hop launch of forward/backward, bracketed with events when profiling is on
 int plan_hop(const b200gf_plan* p, const CsrDev& A, const void* src, int64_t src_ld, void* dst, int64_t dst_ld, int C,
              cudaStream_t st, const ScatterHost* sh = nullptr, const BcastHost* bh = nullptr);
+// the hop chains z_{e,0} = src, z_{e,k} = z_{e,k-1} · op_e (k = 1 .. K-1) of every edge feature e, ops = plan->fwd or
+// plan->bwd.  Hop output t = 1 + e(K-1) + k-1 is written to slot t-1 of buf (n_rows x ld elements per slot); zs / zld
+// receive the T = 1 + E(K-1) terms (pointer, ld), zs[0] = src.
+int hop_chain(const b200gf_plan* p, const std::vector<CsrDev>& ops, const void* src, int64_t src_ld, void* buf, int64_t ld,
+              int C, int K, std::vector<const void*>& zs, std::vector<int64_t>& zld, cudaStream_t st);
 }

@@ -188,14 +188,13 @@ __global__ __launch_bounds__(256) void egate_sddmm_kernel(const int64_t* __restr
   }
 }
 
-inline int grid_for(int64_t total) { return (int)imin64((total + 255) / 256, 132 * 16); }
-
 template <typename T>
 int attention_forward_t(int64_t N, int Bs, const int64_t* rowptr, const int32_t* col, const T* s_src, const T* s_dst,
                         const T* mixer, T* alpha, cudaStream_t st) {
   const int64_t total = N * Bs;
   if (total == 0) return B200GF_OK;
-  egate_softmax_kernel<T><<<grid_for(total), 256, 0, st>>>(rowptr, col, s_src, s_dst, mixer, alpha, Bs, total);
+  egate_softmax_kernel<T><<<grid_for(total, 256, 132 * 16), 256, 0, st>>>(rowptr, col, s_src, s_dst, mixer, alpha, Bs,
+                                                                          total);
   LAUNCH_CHECK();
   return B200GF_OK;
 }
@@ -206,10 +205,11 @@ int attention_backward_t(int64_t N, int Bs, const int64_t* rowptr, const int32_t
                          const T* dalpha, T* dlogit, T* dsig1, T* dsig2, cudaStream_t st) {
   const int64_t total = N * Bs;
   if (total == 0) return B200GF_OK;
-  egate_softmax_bwd_kernel<T><<<grid_for(total), 256, 0, st>>>(rowptr, col, s_src, s_dst, mixer, alpha, dalpha, dlogit,
-                                                               dsig2, Bs, total);
+  const int grid = grid_for(total, 256, 132 * 16);
+  egate_softmax_bwd_kernel<T><<<grid, 256, 0, st>>>(rowptr, col, s_src, s_dst, mixer, alpha, dalpha, dlogit, dsig2, Bs,
+                                                    total);
   LAUNCH_CHECK();
-  egate_colsum_kernel<T><<<grid_for(total), 256, 0, st>>>(rowptrT, permT, dlogit, dsig1, Bs, total);
+  egate_colsum_kernel<T><<<grid, 256, 0, st>>>(rowptrT, permT, dlogit, dsig1, Bs, total);
   LAUNCH_CHECK();
   return B200GF_OK;
 }
@@ -230,11 +230,11 @@ int hop_t(int64_t n_rows, int Bs, int C, const int64_t* rowptr, const int32_t* c
   constexpr int VV = sizeof(T) == 4 ? 4 : 2;                     // one 16-byte access per lane
   if (vec_ok<T, VV>(C, src_ld, dst_ld, src, dst)) {
     const int64_t per_row = cols / VV;
-    egate_hop_kernel<T, VV><<<grid_for(n_rows * per_row), 256, 0, st>>>(rowptr, col, val, pos, gate, g_sb, g_sp, src,
-                                                                       src_ld, dst, dst_ld, C, per_row, n_rows * per_row);
+    egate_hop_kernel<T, VV><<<grid_for(n_rows * per_row, 256, 132 * 16), 256, 0, st>>>(
+        rowptr, col, val, pos, gate, g_sb, g_sp, src, src_ld, dst, dst_ld, C, per_row, n_rows * per_row);
   } else {
-    egate_hop_kernel<T, 1><<<grid_for(n_rows * cols), 256, 0, st>>>(rowptr, col, val, pos, gate, g_sb, g_sp, src, src_ld,
-                                                                    dst, dst_ld, C, cols, n_rows * cols);
+    egate_hop_kernel<T, 1><<<grid_for(n_rows * cols, 256, 132 * 16), 256, 0, st>>>(
+        rowptr, col, val, pos, gate, g_sb, g_sp, src, src_ld, dst, dst_ld, C, cols, n_rows * cols);
   }
   LAUNCH_CHECK();
   return B200GF_OK;
@@ -250,8 +250,8 @@ int hop_backward_t(int64_t N, int Bs, int C, const int64_t* rowptr, const int32_
     if (rc != B200GF_OK) return rc;
   }
   if (dgate && N * Bs > 0) {
-    egate_sddmm_kernel<T><<<grid_for(N * Bs), 256, 0, st>>>(m_rowptr, m_col, m_sval, src, src_ld, ddst, ddst_ld, dgate,
-                                                            d_sb, d_sp, Bs, C, N * Bs);
+    egate_sddmm_kernel<T><<<grid_for(N * Bs, 256, 132 * 16), 256, 0, st>>>(m_rowptr, m_col, m_sval, src, src_ld, ddst,
+                                                                           ddst_ld, dgate, d_sb, d_sp, Bs, C, N * Bs);
     LAUNCH_CHECK();
   }
   return B200GF_OK;
@@ -262,57 +262,17 @@ int hop_backward_t(int64_t N, int Bs, int C, const int64_t* rowptr, const int32_
 
 extern "C" {
 
-int b200gf_egate_attention_forward(int dtype, int64_t N, int64_t nnz, int Bs, const int64_t* rowptr,
-                                   const int32_t* col, const void* s, const void* mixer, void* alpha, void* stream) {
-  using namespace b200gf;
-  if (N < 0 || nnz < 0 || Bs <= 0) return B200GF_EINVAL;
-  if (!rowptr || !s || !mixer || (nnz > 0 && (!col || !alpha))) return B200GF_EINVAL;
-  if (N > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B200GF_F32)
-    return egate::attention_forward_t<float>(N, Bs, rowptr, col, (const float*)s, (const float*)s, (const float*)mixer,
-                                             (float*)alpha, st);
-  if (dtype == B200GF_F64)
-    return egate::attention_forward_t<double>(N, Bs, rowptr, col, (const double*)s, (const double*)s,
-                                              (const double*)mixer, (double*)alpha, st);
-  return B200GF_EUNSUPPORTED;
-}
-
-int b200gf_egate_attention_backward(int dtype, int64_t N, int64_t nnz, int Bs, const int64_t* rowptr,
-                                    const int32_t* col, const int64_t* rowptrT, const int32_t* permT, const void* s,
-                                    const void* mixer, const void* alpha, const void* dalpha, void* dlogit,
-                                    void* dsig1, void* dsig2, void* stream) {
-  using namespace b200gf;
-  if (N < 0 || nnz < 0 || Bs <= 0) return B200GF_EINVAL;
-  if (!rowptr || !rowptrT || !s || !mixer || !dsig1 || !dsig2) return B200GF_EINVAL;
-  if (nnz > 0 && (!col || !permT || !alpha || !dalpha || !dlogit)) return B200GF_EINVAL;
-  if (N > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B200GF_F32)
-    return egate::attention_backward_t<float>(N, Bs, rowptr, col, rowptrT, permT, (const float*)s, (const float*)s,
-                                              (const float*)mixer, (const float*)alpha, (const float*)dalpha, (float*)dlogit, (float*)dsig1,
-                                              (float*)dsig2, st);
-  if (dtype == B200GF_F64)
-    return egate::attention_backward_t<double>(N, Bs, rowptr, col, rowptrT, permT, (const double*)s,
-                                               (const double*)s, (const double*)mixer, (const double*)alpha, (const double*)dalpha,
-                                               (double*)dlogit, (double*)dsig1, (double*)dsig2, st);
-  return B200GF_EUNSUPPORTED;
-}
-
 int b200gf_attention_forward(int dtype, int64_t N, int64_t nnz, int Bs, const int64_t* rowptr, const int32_t* col,
                              const void* s_src, const void* s_dst, const void* mixer, void* alpha, void* stream) {
   using namespace b200gf;
   if (N < 0 || nnz < 0 || Bs <= 0) return B200GF_EINVAL;
   if (!rowptr || !s_src || !s_dst || !mixer || (nnz > 0 && (!col || !alpha))) return B200GF_EINVAL;
   if (N > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B200GF_F32)
-    return egate::attention_forward_t<float>(N, Bs, rowptr, col, (const float*)s_src, (const float*)s_dst,
-                                             (const float*)mixer, (float*)alpha, st);
-  if (dtype == B200GF_F64)
-    return egate::attention_forward_t<double>(N, Bs, rowptr, col, (const double*)s_src, (const double*)s_dst,
-                                              (const double*)mixer, (double*)alpha, st);
-  return B200GF_EUNSUPPORTED;
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return egate::attention_forward_t<T>(N, Bs, rowptr, col, (const T*)s_src, (const T*)s_dst, (const T*)mixer, (T*)alpha,
+                                         (cudaStream_t)stream);
+  });
 }
 
 int b200gf_attention_backward(int dtype, int64_t N, int64_t nnz, int Bs, const int64_t* rowptr, const int32_t* col,
@@ -324,17 +284,26 @@ int b200gf_attention_backward(int dtype, int64_t N, int64_t nnz, int Bs, const i
   if (!rowptr || !rowptrT || !s_src || !s_dst || !mixer || !dsig1 || !dsig2) return B200GF_EINVAL;
   if (nnz > 0 && (!col || !permT || !alpha || !dalpha || !dlogit)) return B200GF_EINVAL;
   if (N > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B200GF_F32)
-    return egate::attention_backward_t<float>(N, Bs, rowptr, col, rowptrT, permT, (const float*)s_src,
-                                              (const float*)s_dst, (const float*)mixer, (const float*)alpha, (const float*)dalpha,
-                                              (float*)dlogit, (float*)dsig1, (float*)dsig2, st);
-  if (dtype == B200GF_F64)
-    return egate::attention_backward_t<double>(N, Bs, rowptr, col, rowptrT, permT, (const double*)s_src,
-                                               (const double*)s_dst, (const double*)mixer, (const double*)alpha,
-                                               (const double*)dalpha, (double*)dlogit, (double*)dsig1, (double*)dsig2,
-                                               st);
-  return B200GF_EUNSUPPORTED;
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return egate::attention_backward_t<T>(N, Bs, rowptr, col, rowptrT, permT, (const T*)s_src, (const T*)s_dst,
+                                          (const T*)mixer, (const T*)alpha, (const T*)dalpha, (T*)dlogit, (T*)dsig1,
+                                          (T*)dsig2, (cudaStream_t)stream);
+  });
+}
+
+// edge gating: the attention softmax with one score array s for both ends of an edge
+int b200gf_egate_attention_forward(int dtype, int64_t N, int64_t nnz, int Bs, const int64_t* rowptr,
+                                   const int32_t* col, const void* s, const void* mixer, void* alpha, void* stream) {
+  return b200gf_attention_forward(dtype, N, nnz, Bs, rowptr, col, s, s, mixer, alpha, stream);
+}
+
+int b200gf_egate_attention_backward(int dtype, int64_t N, int64_t nnz, int Bs, const int64_t* rowptr,
+                                    const int32_t* col, const int64_t* rowptrT, const int32_t* permT, const void* s,
+                                    const void* mixer, const void* alpha, const void* dalpha, void* dlogit,
+                                    void* dsig1, void* dsig2, void* stream) {
+  return b200gf_attention_backward(dtype, N, nnz, Bs, rowptr, col, rowptrT, permT, s, s, mixer, alpha, dalpha, dlogit,
+                                   dsig1, dsig2, stream);
 }
 
 int b200gf_gated_hop_forward(int dtype, int64_t N, int Bs, int C, const int64_t* rowptrT, const int32_t* colT,
@@ -345,14 +314,11 @@ int b200gf_gated_hop_forward(int dtype, int64_t N, int Bs, int C, const int64_t*
   if (!rowptrT || !colT || !valT || !posT || !gate || !src || !dst) return B200GF_EINVAL;
   if (src_ld < (int64_t)Bs * C || dst_ld < (int64_t)Bs * C) return B200GF_EINVAL;
   if (N > INT32_MAX) return B200GF_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B200GF_F32)
-    return egate::hop_t<float>(N, Bs, C, rowptrT, colT, (const float*)valT, posT, (const float*)gate, gate_sb, gate_sp,
-                               (const float*)src, src_ld, (float*)dst, dst_ld, st);
-  if (dtype == B200GF_F64)
-    return egate::hop_t<double>(N, Bs, C, rowptrT, colT, (const double*)valT, posT, (const double*)gate, gate_sb, gate_sp,
-                                (const double*)src, src_ld, (double*)dst, dst_ld, st);
-  return B200GF_EUNSUPPORTED;
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return egate::hop_t<T>(N, Bs, C, rowptrT, colT, (const T*)valT, posT, (const T*)gate, gate_sb, gate_sp, (const T*)src,
+                           src_ld, (T*)dst, dst_ld, (cudaStream_t)stream);
+  });
 }
 
 int b200gf_gated_hop_backward(int dtype, int64_t N, int Bs, int C, const int64_t* rowptr, const int32_t* col,
@@ -366,18 +332,12 @@ int b200gf_gated_hop_backward(int dtype, int64_t N, int Bs, int C, const int64_t
   if (dgate && (!m_rowptr || !m_col || !m_sval || !src || src_ld < (int64_t)Bs * C)) return B200GF_EINVAL;
   if (ddst_ld < (int64_t)Bs * C) return B200GF_EINVAL;
   if (N > INT32_MAX) return B200GF_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B200GF_F32)
-    return egate::hop_backward_t<float>(N, Bs, C, rowptr, col, (const float*)val, pos, m_rowptr, m_col,
-                                        (const float*)m_sval, (const float*)gate, gate_sb, gate_sp, (const float*)src,
-                                        src_ld, (const float*)ddst, ddst_ld, (float*)dsrc, dsrc_ld, (float*)dgate,
-                                        dgate_sb, dgate_sp, st);
-  if (dtype == B200GF_F64)
-    return egate::hop_backward_t<double>(N, Bs, C, rowptr, col, (const double*)val, pos, m_rowptr, m_col,
-                                         (const double*)m_sval, (const double*)gate, gate_sb, gate_sp, (const double*)src,
-                                         src_ld, (const double*)ddst, ddst_ld, (double*)dsrc, dsrc_ld, (double*)dgate,
-                                         dgate_sb, dgate_sp, st);
-  return B200GF_EUNSUPPORTED;
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return egate::hop_backward_t<T>(N, Bs, C, rowptr, col, (const T*)val, pos, m_rowptr, m_col, (const T*)m_sval,
+                                    (const T*)gate, gate_sb, gate_sp, (const T*)src, src_ld, (const T*)ddst, ddst_ld,
+                                    (T*)dsrc, dsrc_ld, (T*)dgate, dgate_sb, dgate_sp, (cudaStream_t)stream);
+  });
 }
 
 }  // extern "C"

@@ -243,8 +243,6 @@ xgrad_kernel(const int64_t* __restrict__ rowptrT, const int32_t* __restrict__ co
   }
 }
 
-inline int grid_for(int64_t total) { return (int)imin64((total + 255) / 256, 132 * 16); }
-
 // 16-byte batch vectors: float data, B a multiple of 4, every operand 16-byte aligned (all row strides are multiples of B)
 template <typename T>
 inline bool vec4_ok(int B, const void* a, const void* b, const void* c, const void* d) {
@@ -265,9 +263,9 @@ int forward_t(int64_t NA, int B, int G, int F, int K, const int64_t* rowptr, con
     const T* prev = k > 0 ? states + (int64_t)((k - 1) % n_states) * chain : nullptr;
     T* cur = k < K - 1 ? states + (int64_t)(k % n_states) * chain : nullptr;
     if (vec4_ok<T>(B, w, xT, states, Y))
-      step_kernel<T, 4><<<grid_for(total / 4), 256, 0, st>>>(rowptr, col, diag, w, prev, xT, cur, Y, (int)NA, B, G, K, k, (int)nnz, total / 4);
+      step_kernel<T, 4><<<grid_for(total / 4, 256, 132 * 16), 256, 0, st>>>(rowptr, col, diag, w, prev, xT, cur, Y, (int)NA, B, G, K, k, (int)nnz, total / 4);
     else
-      step_kernel<T, 1><<<grid_for(total), 256, 0, st>>>(rowptr, col, diag, w, prev, xT, cur, Y, (int)NA, B, G, K, k, (int)nnz, total);
+      step_kernel<T, 1><<<grid_for(total, 256, 132 * 16), 256, 0, st>>>(rowptr, col, diag, w, prev, xT, cur, Y, (int)NA, B, G, K, k, (int)nnz, total);
     LAUNCH_CHECK();
   }
   return B200GF_OK;
@@ -281,7 +279,7 @@ int backward_t(int64_t NA, int B, int G, int F, int K, const int64_t* rowptr, co
   if (chain == 0) return B200GF_OK;
   T* cur = lam;
   T* nxt = lam + chain;
-  adjoint_init_kernel<T><<<grid_for(chain), 256, 0, st>>>(dY, cur, NA, B, G, chain);
+  adjoint_init_kernel<T><<<grid_for(chain, 256, 132 * 16), 256, 0, st>>>(dY, cur, NA, B, G, chain);
   LAUNCH_CHECK();
   const int64_t items = (int64_t)F * G * NA;
   for (int k = K - 1; k >= 0; --k) {
@@ -293,14 +291,14 @@ int backward_t(int64_t NA, int B, int G, int F, int K, const int64_t* rowptr, co
     }
     if (k == 0) break;
     if (vec4_ok<T>(B, dY, lam, lam, dY))
-      adjoint_step_kernel<T, 4><<<grid_for(chain / 4), 256, 0, st>>>(rowptrT, colT, perm, w, dY, cur, nxt, (int)NA, B, G, K, k, (int)nnz, chain / 4);
+      adjoint_step_kernel<T, 4><<<grid_for(chain / 4, 256, 132 * 16), 256, 0, st>>>(rowptrT, colT, perm, w, dY, cur, nxt, (int)NA, B, G, K, k, (int)nnz, chain / 4);
     else
-      adjoint_step_kernel<T, 1><<<grid_for(chain), 256, 0, st>>>(rowptrT, colT, perm, w, dY, cur, nxt, (int)NA, B, G, K, k, (int)nnz, chain);
+      adjoint_step_kernel<T, 1><<<grid_for(chain, 256, 132 * 16), 256, 0, st>>>(rowptrT, colT, perm, w, dY, cur, nxt, (int)NA, B, G, K, k, (int)nnz, chain);
     LAUNCH_CHECK();
     T* tmp = cur; cur = nxt; nxt = tmp;
   }
   const int64_t tx = (int64_t)G * NA * B;
-  xgrad_kernel<T><<<grid_for(tx), 256, 0, st>>>(rowptrT, colT, perm, diag, w, cur, dxT, NA, B, G, F, K, nnz, tx);
+  xgrad_kernel<T><<<grid_for(tx, 256, 132 * 16), 256, 0, st>>>(rowptrT, colT, perm, diag, w, cur, dxT, NA, B, G, F, K, nnz, tx);
   LAUNCH_CHECK();
   return B200GF_OK;
 }
@@ -319,14 +317,11 @@ int b200gf_ev_forward(int dtype, int64_t NA, int B, int G, int F, int K, const i
   if (NA > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
   if (K > 1 && (!states || n_states < 1 || (n_states < K - 1 && n_states != 2))) return B200GF_EINVAL;
   if (K > 2 && n_states == 1) return B200GF_EINVAL;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B200GF_F32)
-    return ev::forward_t<float>(NA, B, G, F, K, rowptr, col, diag, nnz, (const float*)w, (const float*)xT, (float*)states,
-                                n_states < 1 ? 1 : n_states, (float*)Y, st);
-  if (dtype == B200GF_F64)
-    return ev::forward_t<double>(NA, B, G, F, K, rowptr, col, diag, nnz, (const double*)w, (const double*)xT, (double*)states,
-                                 n_states < 1 ? 1 : n_states, (double*)Y, st);
-  return B200GF_EUNSUPPORTED;
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return ev::forward_t<T>(NA, B, G, F, K, rowptr, col, diag, nnz, (const T*)w, (const T*)xT, (T*)states,
+                            n_states < 1 ? 1 : n_states, (T*)Y, (cudaStream_t)stream);
+  });
 }
 
 int b200gf_ev_backward(int dtype, int64_t NA, int B, int G, int F, int K, const int64_t* rowptr, const int32_t* col,
@@ -338,15 +333,11 @@ int b200gf_ev_backward(int dtype, int64_t NA, int B, int G, int F, int K, const 
   if (!rowptr || !col || !rowptrT || !colT || !perm || !xT || !dY || !lam || !dxT || (K > 1 && !states)) return B200GF_EINVAL;
   if (nnz > 0 && (!w || !dw)) return B200GF_EINVAL;
   if (NA > INT32_MAX || nnz > INT32_MAX) return B200GF_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B200GF_F32)
-    return ev::backward_t<float>(NA, B, G, F, K, rowptr, col, rowptrT, colT, perm, diag, nnz, (const float*)w, (const float*)xT,
-                                 (const float*)states, (const float*)dY, (float*)lam, (float*)dw, (float*)dxT, st);
-  if (dtype == B200GF_F64)
-    return ev::backward_t<double>(NA, B, G, F, K, rowptr, col, rowptrT, colT, perm, diag, nnz, (const double*)w,
-                                  (const double*)xT, (const double*)states, (const double*)dY, (double*)lam, (double*)dw,
-                                  (double*)dxT, st);
-  return B200GF_EUNSUPPORTED;
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return ev::backward_t<T>(NA, B, G, F, K, rowptr, col, rowptrT, colT, perm, diag, nnz, (const T*)w, (const T*)xT,
+                             (const T*)states, (const T*)dY, (T*)lam, (T*)dw, (T*)dxT, (cudaStream_t)stream);
+  });
 }
 
 }  // extern "C"

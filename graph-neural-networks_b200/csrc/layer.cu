@@ -55,8 +55,6 @@ __global__ void maxpool_bwd_kernel(const T* __restrict__ dy, int64_t dy_ld, cons
   }
 }
 
-inline int grid_for(int64_t total) { return (int)imin64((total + 255) / 256, 132LL * 16); }
-
 }  // namespace layer
 }  // namespace b200gf
 
@@ -69,14 +67,13 @@ int b200gf_relu_backward(int dtype, const void* y, int64_t y_ld, const void* dy,
   if (!y || !dy || !out || n_rows < 0 || C <= 0 || y_ld < C || dy_ld < C || out_ld < C) return B200GF_EINVAL;
   if (n_rows == 0) return B200GF_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int g = layer::grid_for(n_rows * C);
-  if (dtype == B200GF_F32)
-    layer::relu_bwd_kernel<float><<<g, 256, 0, st>>>((const float*)y, y_ld, (const float*)dy, dy_ld, (float*)out, out_ld, n_rows, C);
-  else if (dtype == B200GF_F64)
-    layer::relu_bwd_kernel<double><<<g, 256, 0, st>>>((const double*)y, y_ld, (const double*)dy, dy_ld, (double*)out, out_ld, n_rows, C);
-  else return B200GF_EUNSUPPORTED;
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  const int g = grid_for(n_rows * C, 256, 132 * 16);
+  return with_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    layer::relu_bwd_kernel<T><<<g, 256, 0, st>>>((const T*)y, y_ld, (const T*)dy, dy_ld, (T*)out, out_ld, n_rows, C);
+    LAUNCH_CHECK();
+    return B200GF_OK;
+  });
 }
 
 int b200gf_maxpool_forward(int dtype, const void* x, int64_t x_ld, int64_t n_in, int C, const int32_t* nb, int64_t n_out,
@@ -85,31 +82,28 @@ int b200gf_maxpool_forward(int dtype, const void* x, int64_t x_ld, int64_t n_in,
   if (n_in > INT32_MAX) return B200GF_EUNSUPPORTED;
   if (n_out == 0) return B200GF_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int g = layer::grid_for(n_out * C);
-  if (dtype == B200GF_F32)
-    layer::maxpool_fwd_kernel<float><<<g, 256, 0, st>>>((const float*)x, x_ld, nb, max_nb, (float*)out, out_ld, argmax, n_out, C);
-  else if (dtype == B200GF_F64)
-    layer::maxpool_fwd_kernel<double><<<g, 256, 0, st>>>((const double*)x, x_ld, nb, max_nb, (double*)out, out_ld, argmax, n_out, C);
-  else return B200GF_EUNSUPPORTED;
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  const int g = grid_for(n_out * C, 256, 132 * 16);
+  return with_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    layer::maxpool_fwd_kernel<T><<<g, 256, 0, st>>>((const T*)x, x_ld, nb, max_nb, (T*)out, out_ld, argmax, n_out, C);
+    LAUNCH_CHECK();
+    return B200GF_OK;
+  });
 }
 
 int b200gf_maxpool_backward(int dtype, const void* dy, int64_t dy_ld, const int32_t* argmax, int64_t n_out, int C,
                             void* dx, int64_t dx_ld, int64_t n_in, void* stream) {
   if (!dy || !argmax || !dx || n_in <= 0 || n_out < 0 || C <= 0 || dy_ld < C || dx_ld < C) return B200GF_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t es = dtype_size(dtype);
-  if (dtype != B200GF_F32 && dtype != B200GF_F64) return B200GF_EUNSUPPORTED;
-  CUDA_TRY(cudaMemsetAsync(dx, 0, (size_t)n_in * dx_ld * es, st));
-  if (n_out == 0) return B200GF_OK;
-  const int g = layer::grid_for(n_out * C);
-  if (dtype == B200GF_F32)
-    layer::maxpool_bwd_kernel<float><<<g, 256, 0, st>>>((const float*)dy, dy_ld, argmax, (float*)dx, dx_ld, n_out, C);
-  else
-    layer::maxpool_bwd_kernel<double><<<g, 256, 0, st>>>((const double*)dy, dy_ld, argmax, (double*)dx, dx_ld, n_out, C);
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  return with_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    CUDA_TRY(cudaMemsetAsync(dx, 0, (size_t)n_in * dx_ld * sizeof(T), st));
+    if (n_out == 0) return B200GF_OK;
+    layer::maxpool_bwd_kernel<T><<<grid_for(n_out * C, 256, 132 * 16), 256, 0, st>>>((const T*)dy, dy_ld, argmax, (T*)dx,
+                                                                                     dx_ld, n_out, C);
+    LAUNCH_CHECK();
+    return B200GF_OK;
+  });
 }
 
 }  // extern "C"

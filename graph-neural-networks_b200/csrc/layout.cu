@@ -56,21 +56,19 @@ static int run_transpose(const T* src, int64_t src_ld, T* dst, int64_t dst_ld, i
 // [C, N] -> [N, ld]; pad columns [C, ld) are zero-filled so every later kernel may read whole padded rows
 int launch_to_node_major(int dtype, const void* src, void* dst, int64_t dst_ld, int64_t N, int C, cudaStream_t st) {
   if (!src || !dst || N < 0 || C <= 0 || dst_ld < C) return B200GF_EINVAL;
-  if (dtype == B200GF_F32)
-    return run_transpose<float>((const float*)src, N, (float*)dst, dst_ld, C, N, dst_ld, st);
-  if (dtype == B200GF_F64)
-    return run_transpose<double>((const double*)src, N, (double*)dst, dst_ld, C, N, dst_ld, st);
-  return B200GF_EUNSUPPORTED;
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return run_transpose<T>((const T*)src, N, (T*)dst, dst_ld, C, N, dst_ld, st);
+  });
 }
 
 // [N, ld] -> [C, N]
 int launch_to_feature_major(int dtype, const void* src, int64_t src_ld, void* dst, int64_t N, int C, cudaStream_t st) {
   if (!src || !dst || N < 0 || C <= 0 || src_ld < C) return B200GF_EINVAL;
-  if (dtype == B200GF_F32)
-    return run_transpose<float>((const float*)src, src_ld, (float*)dst, N, N, C, N, st);
-  if (dtype == B200GF_F64)
-    return run_transpose<double>((const double*)src, src_ld, (double*)dst, N, N, C, N, st);
-  return B200GF_EUNSUPPORTED;
+  return with_dtype(dtype, [&](auto tag) {
+    using T = decltype(tag);
+    return run_transpose<T>((const T*)src, src_ld, (T*)dst, N, N, C, N, st);
+  });
 }
 
 }  // namespace b200gf

@@ -13,17 +13,6 @@ using namespace b200gf;
 
 namespace {
 
-struct Carver {
-  char* base;
-  size_t off = 0;
-  explicit Carver(void* p) : base((char*)p) {}
-  void* take(size_t bytes) {
-    void* r = base ? base + off : nullptr;
-    off += align_up(bytes, 256);
-    return r;
-  }
-};
-
 struct FwdWs {
   void* xn = nullptr;   // node-major copy of x (only when x arrives feature-major)
   void* z = nullptr;    // E*(K-1) hop outputs, each [n_cols, ldc]
@@ -98,6 +87,28 @@ int plan_hop(const b200gf_plan* p, const CsrDev& A, const void* src, int64_t src
   }
   return rc;
 }
+
+int hop_chain(const b200gf_plan* p, const std::vector<CsrDev>& ops, const void* src, int64_t src_ld, void* buf, int64_t ld,
+              int C, int K, std::vector<const void*>& zs, std::vector<int64_t>& zld, cudaStream_t st) {
+  const size_t slot = (size_t)p->n_rows * ld * dtype_size(p->dtype);
+  zs.assign(1 + p->E * (K - 1), nullptr);
+  zld.assign(1 + p->E * (K - 1), ld);
+  zs[0] = src;
+  zld[0] = src_ld;
+  for (int e = 0; e < p->E; ++e) {
+    const void* prev = src;
+    int64_t prev_ld = src_ld;
+    for (int k = 1; k < K; ++k) {
+      const int t = 1 + e * (K - 1) + (k - 1);
+      void* dst = (char*)buf + (t - 1) * slot;
+      if (int rc = plan_hop(p, ops[e], prev, prev_ld, dst, ld, C, st)) return rc;
+      zs[t] = dst;
+      prev = dst;
+      prev_ld = ld;
+    }
+  }
+  return B200GF_OK;
+}
 }  // namespace b200gf
 
 extern "C" {
@@ -150,18 +161,16 @@ static int forward_impl(const b200gf_plan* plan, const void* x, int x_layout, in
   if (C > INT32_MAX || CF > INT32_MAX) return B200GF_EUNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
   const int dt = plan->dtype;
-  const size_t es = dtype_size(dt);
   const int E = plan->E;
   const int T = 1 + E * (K - 1);
   if (N == 0) return B200GF_OK;
 
   // carve with the caller's actual layouts (never larger than what workspace_bytes() reported)
-  if (((uintptr_t)workspace & 255) != 0 && workspace) return B200GF_EINVAL;
   FwdWs w = carve_fwd(plan, workspace, B, G, F, K, x_layout, y_layout);
-  if (w.bytes > workspace_bytes || (!workspace && w.bytes > 0)) return B200GF_EWORKSPACE;
+  int rc;
+  if ((rc = check_workspace(workspace, w.bytes, workspace_bytes, false))) return rc;
   const int64_t ldc = padded_ld(C, dt), ldf = padded_ld(CF, dt);
 
-  int rc;
   const void* x0 = x;
   int64_t x0_ld = x_ld;
   if (x_layout == B200GF_FEATURE_MAJOR) {
@@ -169,26 +178,9 @@ static int forward_impl(const b200gf_plan* plan, const void* x, int x_layout, in
     x0 = w.xn;
     x0_ld = ldc;
   }
-  std::vector<const void*> zs(T);
-  std::vector<int64_t> zld(T);
-  zs[0] = x0;
-  zld[0] = x0_ld;
-  for (int e = 0; e < E; ++e) {
-    std::vector<void*> chain(K > 1 ? K - 1 : 0);
-    for (int k = 1; k < K; ++k) {
-      const int t = 1 + e * (K - 1) + (k - 1);
-      chain[k - 1] = (char*)w.z + (size_t)(t - 1) * N * ldc * es;
-      zs[t] = chain[k - 1];
-      zld[t] = ldc;
-    }
-    const void* prev = x0;
-    int64_t prev_ld = x0_ld;
-    for (int k = 1; k < K; ++k) {
-      if ((rc = plan_hop(plan, plan->fwd[e], prev, prev_ld, chain[k - 1], ldc, (int)C, st))) return rc;
-      prev = chain[k - 1];
-      prev_ld = ldc;
-    }
-  }
+  std::vector<const void*> zs;
+  std::vector<int64_t> zld;
+  if ((rc = hop_chain(plan, plan->fwd, x0, x0_ld, w.z, ldc, (int)C, K, zs, zld, st))) return rc;
   void* yo = y_layout == B200GF_NODE_MAJOR ? y : w.yn;
   const int64_t yo_ld = y_layout == B200GF_NODE_MAJOR ? y_ld : ldf;
   if (tc_contract_eligible(dt, N, B, G, F, T, zs.data(), zld.data(), yo, yo_ld, 0)) {
@@ -238,13 +230,12 @@ int b200gf_backward(const b200gf_plan* plan, const void* dy, int dy_layout, int6
   const size_t es = dtype_size(dt);
   const int E = plan->E;
   const int T = 1 + E * (K - 1);
-  if (((uintptr_t)workspace & 255) != 0 && workspace) return B200GF_EINVAL;
   const bool any_fm = dy_layout == B200GF_FEATURE_MAJOR || x_layout == B200GF_FEATURE_MAJOR ||
                       (dx && dx_layout == B200GF_FEATURE_MAJOR);
   BwdWs w = carve_bwd(plan, workspace, B, G, F, K, any_fm ? B200GF_FEATURE_MAJOR : B200GF_NODE_MAJOR);
-  if (w.bytes > workspace_bytes || !workspace) return B200GF_EWORKSPACE;
-  const int64_t ldc = padded_ld(C, dt), ldf = padded_ld(CF, dt);
   int rc;
+  if ((rc = check_workspace(workspace, w.bytes, workspace_bytes, true))) return rc;
+  const int64_t ldc = padded_ld(C, dt), ldf = padded_ld(CF, dt);
   if (N == 0) {
     CUDA_TRY(cudaMemsetAsync(dh, 0, (size_t)F * E * K * G * es, st));
     if (dbias && !bias_per_node) CUDA_TRY(cudaMemsetAsync(dbias, 0, (size_t)F * es, st));
@@ -266,26 +257,9 @@ int b200gf_backward(const b200gf_plan* plan, const void* dy, int dy_layout, int6
     x0_ld = ldc;
   }
 
-  std::vector<const void*> vs(T);
-  std::vector<int64_t> vld(T);
-  vs[0] = dy0;
-  vld[0] = dy0_ld;
-  for (int e = 0; e < E; ++e) {
-    std::vector<void*> chain(K > 1 ? K - 1 : 0);
-    for (int k = 1; k < K; ++k) {
-      const int t = 1 + e * (K - 1) + (k - 1);
-      chain[k - 1] = (char*)w.v + (size_t)(t - 1) * N * ldf * es;
-      vs[t] = chain[k - 1];
-      vld[t] = ldf;
-    }
-    const void* prev = dy0;
-    int64_t prev_ld = dy0_ld;
-    for (int k = 1; k < K; ++k) {
-      if ((rc = plan_hop(plan, plan->bwd[e], prev, prev_ld, chain[k - 1], ldf, (int)CF, st))) return rc;
-      prev = chain[k - 1];
-      prev_ld = ldf;
-    }
-  }
+  std::vector<const void*> vs;
+  std::vector<int64_t> vld;
+  if ((rc = hop_chain(plan, plan->bwd, dy0, dy0_ld, w.v, ldf, (int)CF, K, vs, vld, st))) return rc;
   if (dx) {
     void* dxo = dx_layout == B200GF_NODE_MAJOR ? dx : w.dxn;
     const int64_t dxo_ld = dx_layout == B200GF_NODE_MAJOR ? dx_ld : ldc;

@@ -14,8 +14,6 @@
 //           writes one partial per piece, pass 2 sums a tap's pieces in order and unpacks to h's layout [F,E,K,G,M].
 #include "../common.cuh"
 
-#include <algorithm>
-
 using namespace b200gf;
 
 namespace {
@@ -24,12 +22,10 @@ constexpr int NV_THREADS = 128;                  // contraction block
 constexpr int NV_BT = 8;                         // batch lanes a contraction thread keeps in registers
 constexpr size_t NV_SMEM = 48 * 1024;            // staged tap rows (the default dynamic shared-memory limit)
 constexpr int NV_TG_THREADS = 256;               // tap-gradient block
-constexpr int NV_PIECES_TARGET = 1024;           // a tap shared by all N nodes is cut into about this many pieces
 
-int64_t nv_chunk(int64_t N) { return std::max<int64_t>(32, (N + NV_PIECES_TARGET - 1) / NV_PIECES_TARGET); }
-
-// sum_m ceil(cnt_m / chunk) < N / chunk + (number of non-empty taps)
-int64_t nv_pieces_bound(int64_t N, int64_t M) { return N / nv_chunk(N) + std::min(M, N) + 1; }
+// a tap shared by all N nodes is cut into pieces of piece_rows(N) nodes: sum_m ceil(cnt_m / chunk) < N / chunk + (number
+// of non-empty taps)
+int64_t nv_pieces_bound(int64_t N, int64_t M) { return N / piece_rows(N) + std::min(M, N) + 1; }
 
 // ---------------------------------------------------------------------------------------------------------------
 // pack: h [F][E][K][G][M] -> W [M][T][G][F]
@@ -243,19 +239,11 @@ __global__ void nv_add_kernel(T* __restrict__ dst, int64_t dst_ld, const T* __re
   }
 }
 
-int grid_for(int64_t total, int threads, int sm_count) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((total + threads - 1) / threads, (int64_t)sm_count * 8));
-}
-
 int launch_nv_contract(int dt, int sm_count, const void* const* zs, const int64_t* z_ld, int T_terms, int t_first,
                        int T_all, int64_t n_rows, int B, int P, int Q, int transposed, const void* W,
                        const int32_t* node_tap, const void* bias, int bias_per_node, const void* add, int64_t add_ld,
                        void* out, int64_t out_ld, cudaStream_t st) {
-  TermList tl;
-  for (int i = 0; i < T_terms; ++i) {
-    tl.ptr[i] = zs[i];
-    tl.ld[i] = z_ld[i];
-  }
+  const TermList tl = make_terms(zs, z_ld, T_terms);
   const size_t es = dtype_size(dt);
   const int R = T_terms * P;
   const int rows_fit = (int)std::min<size_t>((size_t)R, NV_SMEM / ((size_t)Q * es));
@@ -281,23 +269,14 @@ int launch_nv_contract(int dt, int sm_count, const void* const* zs, const int64_
 
 int launch_nv_add(int dt, int sm_count, void* dst, int64_t dst_ld, const void* src, int64_t src_ld, int64_t n_rows, int C,
                   cudaStream_t st) {
-  const int grid = grid_for(n_rows * C, 256, sm_count);
-  if (dt == B200GF_F32) nv_add_kernel<float><<<grid, 256, 0, st>>>((float*)dst, dst_ld, (const float*)src, src_ld, n_rows, C);
-  else nv_add_kernel<double><<<grid, 256, 0, st>>>((double*)dst, dst_ld, (const double*)src, src_ld, n_rows, C);
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  const int grid = grid_for(n_rows * C, 256, sm_count * 8);
+  return with_dtype(dt, [&](auto tag) -> int {
+    using T = decltype(tag);
+    nv_add_kernel<T><<<grid, 256, 0, st>>>((T*)dst, dst_ld, (const T*)src, src_ld, n_rows, C);
+    LAUNCH_CHECK();
+    return B200GF_OK;
+  });
 }
-
-struct Carver {
-  char* base;
-  size_t off = 0;
-  explicit Carver(void* p) : base((char*)p) {}
-  void* take(size_t bytes) {
-    void* r = base ? base + off : nullptr;
-    off += align_up(bytes, 256);
-    return r;
-  }
-};
 
 struct NvWs {
   void* z = nullptr;        // E(K-1) hop outputs Z_{e,k}, each [N, ldc]
@@ -337,32 +316,6 @@ NvWs carve_nv(const b200gf_plan* p, void* ws, int B, int G, int F, int K, int64_
   return w;
 }
 
-// Z_{e,k} = Z_{e,k-1} · S_e into the workspace; zs / zld receive the T terms (zs[0] = x)
-int nv_hops(const b200gf_plan* plan, const void* x, int64_t x_ld, void* zbuf, int64_t ldc, int C, int K,
-            std::vector<const void*>& zs, std::vector<int64_t>& zld, cudaStream_t st) {
-  const int E = plan->E;
-  const size_t es = dtype_size(plan->dtype);
-  const int64_t N = plan->n_rows;
-  zs.assign(1 + E * (K - 1), nullptr);
-  zld.assign(1 + E * (K - 1), ldc);
-  zs[0] = x;
-  zld[0] = x_ld;
-  for (int e = 0; e < E; ++e) {
-    const void* prev = x;
-    int64_t prev_ld = x_ld;
-    for (int k = 1; k < K; ++k) {
-      const int t = 1 + e * (K - 1) + (k - 1);
-      void* dst = (char*)zbuf + (size_t)(t - 1) * N * ldc * es;
-      int rc = plan_hop(plan, plan->fwd[e], prev, prev_ld, dst, ldc, C, st);
-      if (rc) return rc;
-      zs[t] = dst;
-      prev = dst;
-      prev_ld = ldc;
-    }
-  }
-  return B200GF_OK;
-}
-
 bool nv_bad_dims(const b200gf_plan* plan, int B, int G, int F, int K, int64_t M) {
   if (!plan || B <= 0 || G <= 0 || F <= 0 || K <= 0 || M <= 0) return true;
   return plan->n_rows != plan->n_cols;                 // partitioned plans are not supported here
@@ -374,14 +327,14 @@ extern "C" {
 
 int b200gf_nv_pack_taps(int dtype, const void* h, void* W, int F, int E, int K, int G, int64_t M, void* stream) {
   if (!h || !W || F <= 0 || E <= 0 || K <= 0 || G <= 0 || M <= 0) return B200GF_EINVAL;
-  if (dtype != B200GF_F32 && dtype != B200GF_F64) return B200GF_EUNSUPPORTED;
   const int64_t total = M * (1 + E * (K - 1)) * (int64_t)G * F;
-  const int grid = grid_for(total, 256, 132);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B200GF_F32) nv_pack_taps_kernel<float><<<grid, 256, 0, st>>>((const float*)h, (float*)W, F, E, K, G, M);
-  else nv_pack_taps_kernel<double><<<grid, 256, 0, st>>>((const double*)h, (double*)W, F, E, K, G, M);
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  const int grid = grid_for(total, 256, 132 * 8);
+  return with_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    nv_pack_taps_kernel<T><<<grid, 256, 0, (cudaStream_t)stream>>>((const T*)h, (T*)W, F, E, K, G, M);
+    LAUNCH_CHECK();
+    return B200GF_OK;
+  });
 }
 
 size_t b200gf_nv_workspace_bytes(const b200gf_plan* plan, int B, int G, int F, int K, int64_t M, int backward) {
@@ -400,16 +353,15 @@ int b200gf_nv_forward(const b200gf_plan* plan, const void* x, int64_t x_ld, cons
   if (C > INT32_MAX || CF > INT32_MAX) return B200GF_EUNSUPPORTED;
   const int T = 1 + plan->E * (K - 1);
   if (T > TermList::MAX_TERMS) return B200GF_EUNSUPPORTED;
-  if (workspace && ((uintptr_t)workspace & 255) != 0) return B200GF_EINVAL;
   NvWs w = carve_nv(plan, workspace, B, G, F, K, M, false);
-  if (w.bytes > workspace_bytes || (!workspace && w.bytes > 0)) return B200GF_EWORKSPACE;
+  int rc;
+  if ((rc = check_workspace(workspace, w.bytes, workspace_bytes, false))) return rc;
   if (N == 0) return B200GF_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int dt = plan->dtype;
   std::vector<const void*> zs;
   std::vector<int64_t> zld;
-  int rc = nv_hops(plan, x, x_ld, w.z, padded_ld(C, dt), (int)C, K, zs, zld, st);
-  if (rc) return rc;
+  if ((rc = hop_chain(plan, plan->fwd, x, x_ld, w.z, padded_ld(C, dt), (int)C, K, zs, zld, st))) return rc;
   return launch_nv_contract(dt, plan->sm_count, zs.data(), zld.data(), T, 0, T, N, B, G, F, 0, W, node_tap, bias,
                             bias_per_node, nullptr, 0, y, y_ld, st);
 }
@@ -428,9 +380,9 @@ int b200gf_nv_backward(const b200gf_plan* plan, const void* dy, int64_t dy_ld, c
   const int E = plan->E;
   const int T = 1 + E * (K - 1);
   if (T > TermList::MAX_TERMS) return B200GF_EUNSUPPORTED;
-  if (!workspace || ((uintptr_t)workspace & 255) != 0) return workspace ? B200GF_EINVAL : B200GF_EWORKSPACE;
   NvWs w = carve_nv(plan, workspace, B, G, F, K, M, true);
-  if (w.bytes > workspace_bytes) return B200GF_EWORKSPACE;
+  int rc;
+  if ((rc = check_workspace(workspace, w.bytes, workspace_bytes, true))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int dt = plan->dtype;
   const size_t es = dtype_size(dt);
@@ -441,34 +393,26 @@ int b200gf_nv_backward(const b200gf_plan* plan, const void* dy, int64_t dy_ld, c
     return B200GF_OK;
   }
   const int64_t ldc = padded_ld(C, dt);
-  int rc;
 
   // dh: Z_t recomputed from x, segmented two-pass reduction over the members of each tap
   std::vector<const void*> zs;
   std::vector<int64_t> zld;
-  if ((rc = nv_hops(plan, x, x_ld, w.z, ldc, (int)C, K, zs, zld, st))) return rc;
-  const int64_t chunk = nv_chunk(N);
+  if ((rc = hop_chain(plan, plan->fwd, x, x_ld, w.z, ldc, (int)C, K, zs, zld, st))) return rc;
+  const int64_t chunk = piece_rows(N);
   nv_piece_scan_kernel<<<1, NV_SCAN_THREADS, 0, st>>>(tap_rowptr, M, chunk, w.piece_ptr);
   LAUNCH_CHECK();
-  TermList tl;
-  for (int t = 0; t < T; ++t) {
-    tl.ptr[t] = zs[t];
-    tl.ld[t] = zld[t];
-  }
+  const TermList tl = make_terms(zs.data(), zld.data(), T);
   const dim3 pgrid((unsigned)nv_pieces_bound(N, M), (unsigned)T);
-  const int rgrid = grid_for((int64_t)F * E * K * G * M, 256, sms);
-  if (dt == B200GF_F32) {
-    nv_tap_grad_partial_kernel<float><<<pgrid, NV_TG_THREADS, 0, st>>>(tl, T, B, G, F, (const float*)dy, dy_ld, tap_rowptr,
-                                                                      tap_nodes, w.piece_ptr, M, chunk, (float*)w.partial);
-    nv_tap_grad_reduce_kernel<float><<<rgrid, 256, 0, st>>>((const float*)w.partial, w.piece_ptr, M, F, E, K, G, (float*)dh);
-  } else {
-    nv_tap_grad_partial_kernel<double><<<pgrid, NV_TG_THREADS, 0, st>>>(tl, T, B, G, F, (const double*)dy, dy_ld,
-                                                                       tap_rowptr, tap_nodes, w.piece_ptr, M, chunk,
-                                                                       (double*)w.partial);
-    nv_tap_grad_reduce_kernel<double><<<rgrid, 256, 0, st>>>((const double*)w.partial, w.piece_ptr, M, F, E, K, G,
-                                                            (double*)dh);
-  }
-  LAUNCH_CHECK_N(2);
+  const int rgrid = grid_for((int64_t)F * E * K * G * M, 256, sms * 8);
+  rc = with_dtype(dt, [&](auto tag) -> int {
+    using Ty = decltype(tag);
+    nv_tap_grad_partial_kernel<Ty><<<pgrid, NV_TG_THREADS, 0, st>>>(tl, T, B, G, F, (const Ty*)dy, dy_ld, tap_rowptr,
+                                                                   tap_nodes, w.piece_ptr, M, chunk, (Ty*)w.partial);
+    nv_tap_grad_reduce_kernel<Ty><<<rgrid, 256, 0, st>>>((const Ty*)w.partial, w.piece_ptr, M, F, E, K, G, (Ty*)dh);
+    LAUNCH_CHECK_N(2);
+    return B200GF_OK;
+  });
+  if (rc) return rc;
 
   // dx by Horner: per e, buf = dz_{e,K-1}; buf = dz_{e,k} + BWD(buf) for k = K-2 .. 1; chain_e = BWD(buf)
   if (dx) {

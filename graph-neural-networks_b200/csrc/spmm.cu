@@ -268,9 +268,9 @@ int launch_hop(int dtype, int sm_count, int64_t l2_bytes, const CsrDev& A, int64
   if (sh && (sh->n_peers < 0 || sh->n_peers > MAX_PEERS)) return B200GF_EINVAL;
   if (bh && (bh->n_peers < 0 || bh->n_peers > MAX_PEERS || (bh->n_peers > 0 && bh->out_ld < C))) return B200GF_EINVAL;
   if (bh && bh->n_peers == 0 && !(sh && sh->n_peers > 0)) return B200GF_EINVAL;   // no all-gather only in the grid epilogue
-  if (dtype == B200GF_F32) return launch_typed<float>(sm_count, l2_bytes, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
-  if (dtype == B200GF_F64) return launch_typed<double>(sm_count, l2_bytes, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
-  return B200GF_EUNSUPPORTED;
+  return with_dtype(dtype, [&](auto tag) {
+    return launch_typed<decltype(tag)>(sm_count, l2_bytes, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
+  });
 }
 
 // all-gather of an existing node-major row block (the k = 0 term x): every rank's full-height matrix gets these rows

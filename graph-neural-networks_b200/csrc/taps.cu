@@ -39,15 +39,12 @@ int launch_pack_taps(int dtype, const void* h, void* W, int F, int E, int K, int
                      cudaStream_t st) {
   if (!h || !W || F <= 0 || E <= 0 || K <= 0 || G <= 0) return B200GF_EINVAL;
   const int64_t total = (int64_t)(1 + E * (K - 1)) * G * F;
-  const int threads = 256;
-  const int blocks = (int)b200gf::imin64((total + threads - 1) / threads, 132 * 8);
-  if (dtype == B200GF_F32)
-    pack_taps_kernel<float><<<blocks, threads, 0, st>>>((const float*)h, (float*)W, F, E, K, G, transpose_taps);
-  else if (dtype == B200GF_F64)
-    pack_taps_kernel<double><<<blocks, threads, 0, st>>>((const double*)h, (double*)W, F, E, K, G, transpose_taps);
-  else return B200GF_EUNSUPPORTED;
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  return with_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    pack_taps_kernel<T><<<grid_for(total, 256, 132 * 8), 256, 0, st>>>((const T*)h, (T*)W, F, E, K, G, transpose_taps);
+    LAUNCH_CHECK();
+    return B200GF_OK;
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -160,14 +157,15 @@ int launch_tap_contract(int dtype, int64_t n_rows, int B, int P, int Q, int T, c
     const void* Wt = (const char*)W + (size_t)t0 * P * Q * es;
     const void* bb = t0 == 0 ? bias : nullptr;
     const int acc = ((t0 == 0) ? (accumulate ? 1 : 0) : 1) | ((act && t0 + TermList::MAX_TERMS >= T) ? 2 : 0);
-    if (dtype == B200GF_F32)
-      tap_contract_kernel<float><<<grid, 256, 0, st>>>(tl, tn, (const float*)Wt, (const float*)bb, bias_per_node,
-                                                       (float*)out, out_ld, n_rows, B, P, Q, acc);
-    else if (dtype == B200GF_F64)
-      tap_contract_kernel<double><<<grid, 256, 0, st>>>(tl, tn, (const double*)Wt, (const double*)bb, bias_per_node,
-                                                        (double*)out, out_ld, n_rows, B, P, Q, acc);
-    else return B200GF_EUNSUPPORTED;
-    LAUNCH_CHECK();
+    // the dtype is looked at only here, after this group's terms are checked
+    const int rc = with_dtype(dtype, [&](auto tag) -> int {
+      using Ty = decltype(tag);
+      tap_contract_kernel<Ty><<<grid, 256, 0, st>>>(tl, tn, (const Ty*)Wt, (const Ty*)bb, bias_per_node, (Ty*)out, out_ld,
+                                                    n_rows, B, P, Q, acc);
+      LAUNCH_CHECK();
+      return B200GF_OK;
+    });
+    if (rc) return rc;
   }
   return B200GF_OK;
 }
@@ -443,24 +441,22 @@ int launch_tap_grad(int dtype, int64_t n_rows, int B, int P, int Q, int T, const
       }
       continue;
     }
-    if (dtype == B200GF_F32)
-      tap_grad_partial_kernel<float><<<grid, 256, 0, st>>>((const float*)A, a_ld, tl, n_rows, B, P, Q,
-                                                           g.rows_per_chunk, g.q_tiles, (float*)part, T);
-    else
-      tap_grad_partial_kernel<double><<<grid, 256, 0, st>>>((const double*)A, a_ld, tl, n_rows, B, P, Q,
-                                                            g.rows_per_chunk, g.q_tiles, (double*)part, T);
-    LAUNCH_CHECK();
+    const int rc = with_dtype(dtype, [&](auto tag) -> int {
+      using Ty = decltype(tag);
+      tap_grad_partial_kernel<Ty><<<grid, 256, 0, st>>>((const Ty*)A, a_ld, tl, n_rows, B, P, Q, g.rows_per_chunk,
+                                                        g.q_tiles, (Ty*)part, T);
+      LAUNCH_CHECK();
+      return B200GF_OK;
+    });
+    if (rc) return rc;
   }
-  const int64_t total = (int64_t)T * P * Q;
-  const int blocks = (int)b200gf::imin64((total + 255) / 256, 132 * 8);
-  if (dtype == B200GF_F32)
-    tap_grad_reduce_kernel<float><<<blocks, 256, 0, st>>>((const float*)scratch, g.n_chunks, T, P, Q, (float*)dW,
-                                                          out_mode, E, K);
-  else
-    tap_grad_reduce_kernel<double><<<blocks, 256, 0, st>>>((const double*)scratch, g.n_chunks, T, P, Q, (double*)dW,
-                                                           out_mode, E, K);
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  const int blocks = grid_for((int64_t)T * P * Q, 256, 132 * 8);
+  return with_dtype(dtype, [&](auto tag) -> int {
+    using Ty = decltype(tag);
+    tap_grad_reduce_kernel<Ty><<<blocks, 256, 0, st>>>((const Ty*)scratch, g.n_chunks, T, P, Q, (Ty*)dW, out_mode, E, K);
+    LAUNCH_CHECK();
+    return B200GF_OK;
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -563,13 +559,12 @@ int launch_bias_grad(int dtype, int64_t n_rows, int B, int F, const void* dy, in
   if (bias_per_node) {
     const int64_t total = n_rows * F;
     if (total == 0) return B200GF_OK;
-    const int blocks = (int)b200gf::imin64((total + 255) / 256, 132 * 8);
-    if (dtype == B200GF_F32)
-      bias_grad_node_kernel<float><<<blocks, 256, 0, st>>>((const float*)dy, dy_ld, n_rows, B, F, (float*)dbias);
-    else
-      bias_grad_node_kernel<double><<<blocks, 256, 0, st>>>((const double*)dy, dy_ld, n_rows, B, F, (double*)dbias);
-    LAUNCH_CHECK();
-    return B200GF_OK;
+    return with_dtype(dtype, [&](auto tag) -> int {
+      using T = decltype(tag);
+      bias_grad_node_kernel<T><<<grid_for(total, 256, 132 * 8), 256, 0, st>>>((const T*)dy, dy_ld, n_rows, B, F, (T*)dbias);
+      LAUNCH_CHECK();
+      return B200GF_OK;
+    });
   }
   if (!scratch || scratch_bytes < bias_grad_scratch_bytes(dtype, n_rows, B, F)) return B200GF_EWORKSPACE;
   const int n_chunks = (int)((n_rows + BG_ROWS - 1) / BG_ROWS);
