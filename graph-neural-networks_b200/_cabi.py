@@ -31,6 +31,7 @@ _SIGNATURES = {
     "b200gf_plan_destroy": (None, [c_vp]),
     "b200gf_plan_info": (c_i64, [c_vp, c_int]),
     "b200gf_plan_set_l2_bytes": (c_int, [c_vp, c_i64]),
+    "b200gf_plan_set_hop_windows": (c_int, [c_vp, c_i64]),
     "b200gf_forward": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp, c_vp, c_int, c_vp, c_int, c_i64, c_vp, c_sz,
                                c_int, c_int, c_int, c_int, c_vp]),
     "b200gf_forward_act": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp, c_vp, c_int, c_vp, c_int, c_i64, c_vp, c_sz,

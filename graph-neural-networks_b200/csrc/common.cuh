@@ -41,6 +41,14 @@ struct CsrDev {
   // most non-zeros lie far from the diagonal, so a hop's gathers spread over the whole source (hop_chunk_lanes);
   // set by b200gf_plan_create, which sees the host CSR
   bool spread = false;
+  // window-major copy of the operator (b200gf_plan_set_hop_windows): window w holds the entries whose column lies in
+  // [w * win_rows, (w + 1) * win_rows), as a full-height CSR with offsets win_rowptr32[w * (n_rows + 1) ..] into the
+  // shared win_col / win_val (window 0's entries first).  Columns stay global.  win_rows == 0: no copy.
+  int64_t win_rows = 0;
+  int n_win = 0;
+  int32_t* win_rowptr32 = nullptr;  // [n_win * (n_rows + 1)]
+  int32_t* win_col = nullptr;       // [nnz]
+  void* win_val = nullptr;          // [nnz] of dtype
 };
 
 inline size_t dtype_size(int dtype) { return dtype == B200GF_F64 ? 8 : 4; }
@@ -109,6 +117,8 @@ struct BcastHost {
 int launch_hop(int dtype, int sm_count, int64_t l2_bytes, const CsrDev& A, int64_t n_rows, const void* src,
                int64_t src_ld, void* dst, int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh = nullptr,
                const BcastHost* bh = nullptr);
+// rows per source window of the default window-major operator copy, 0 for none (spmm.cu)
+int64_t hop_window_rows(int64_t n_src, int64_t l2_bytes, bool spread);
 int launch_scatter_rows(int dtype, const void* src, int64_t src_ld, int64_t n_rows, int C, cudaStream_t st,
                         const ScatterHost* sh);
 int launch_bcast_rows(int dtype, const void* src, int64_t src_ld, int64_t n_rows, int C, cudaStream_t st,
@@ -179,6 +189,7 @@ struct b200gf_plan {
   int64_t l2_bytes = 0;   // device L2 size the hops size their column chunks against (b200gf_plan_set_l2_bytes)
   bool symmetric = false;
   bool has_bwd = false;
+  bool from_gso = false;      // built by b200gf_plan_create: the only plans that take window-major operator copies
   std::vector<b200gf::CsrDev> fwd;  // CSR of S_e^T rows: forward shift gather operator
   std::vector<b200gf::CsrDev> bwd;  // CSR of S_e rows  : backward shift gather operator
   // measurement hook (b200gf_profile_hops): event pairs around hop launches

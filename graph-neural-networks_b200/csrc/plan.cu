@@ -128,13 +128,91 @@ struct DeviceGuard {
   ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
+void free_windows(CsrDev& D) {
+  if (D.owned) {
+    if (D.win_rowptr32) cudaFree(D.win_rowptr32);
+    if (D.win_col) cudaFree(D.win_col);
+    if (D.win_val) cudaFree(D.win_val);
+  }
+  D.win_rowptr32 = nullptr; D.win_col = nullptr; D.win_val = nullptr;
+  D.win_rows = 0; D.n_win = 0;
+}
+
 void free_csr(CsrDev& D) {
+  free_windows(D);
   if (!D.owned) return;
   if (D.rowptr) cudaFree(D.rowptr);
   if (D.rowptr32) cudaFree(D.rowptr32);
   if (D.col) cudaFree(D.col);
   if (D.val) cudaFree(D.val);
   D.rowptr = nullptr; D.rowptr32 = nullptr; D.col = nullptr; D.val = nullptr;
+}
+
+// Window-major copy of a square operator (CsrDev::win_*): a counting sort of the entries by (column window, row) that
+// keeps each row's entry order.  O(nnz + W * N) on the host.  The new copy is built aside and replaces D's only once it
+// is complete: on any error D keeps what it had, and nothing half-built or allocated is left behind.
+int build_windows(const HostCsr& A, int64_t N, size_t es, int64_t R, CsrDev& D) {
+  const int64_t nnz = A.rowptr[N];
+  if (N == 0 || R <= 0) return B200GF_EUNSUPPORTED;
+  const int64_t W = (N - 1) / R + 1;
+  if (nnz >= (int64_t)INT32_MAX || W * (N + 1) >= (int64_t)INT32_MAX) return B200GF_EUNSUPPORTED;
+  std::vector<int32_t> rp, col, cursor;
+  std::vector<unsigned char> val;
+  try {
+    rp.assign((size_t)(W * (N + 1)), 0);
+    col.resize((size_t)nnz);
+    val.resize((size_t)nnz * es);
+    cursor.resize((size_t)(W * N));
+  } catch (const std::bad_alloc&) {
+    return B200GF_ENOMEM;
+  }
+  // count into rp[w * (N + 1) + i + 1], then an exclusive scan in window-major order gives every row's start
+  for (int64_t i = 0; i < N; ++i)
+    for (int64_t j = A.rowptr[i]; j < A.rowptr[i + 1]; ++j) rp[(size_t)((A.col[j] / R) * (N + 1) + i + 1)]++;
+  int32_t run = 0;
+  for (int64_t w = 0; w < W; ++w) {
+    int32_t* r = rp.data() + w * (N + 1);
+    r[0] = run;
+    for (int64_t i = 1; i <= N; ++i) r[i] += r[i - 1];
+    run = r[N];
+  }
+  for (int64_t w = 0; w < W; ++w)
+    for (int64_t i = 0; i < N; ++i) cursor[(size_t)(w * N + i)] = rp[(size_t)(w * (N + 1) + i)];
+  for (int64_t i = 0; i < N; ++i) {
+    for (int64_t j = A.rowptr[i]; j < A.rowptr[i + 1]; ++j) {
+      const int32_t dst = cursor[(size_t)((A.col[j] / R) * N + i)]++;
+      col[dst] = A.col[j];
+      std::memcpy(&val[(size_t)dst * es], &A.val[(size_t)j * es], es);
+    }
+  }
+  CsrDev nw;   // owned
+  const auto upload_copy = [&]() -> int {
+    if (cudaMalloc(&nw.win_rowptr32, rp.size() * sizeof(int32_t)) != cudaSuccess) return B200GF_ENOMEM;
+    if (cudaMalloc(&nw.win_col, (size_t)(nnz + 1) * sizeof(int32_t)) != cudaSuccess) return B200GF_ENOMEM;
+    if (cudaMalloc(&nw.win_val, (size_t)(nnz + 1) * es) != cudaSuccess) return B200GF_ENOMEM;
+    CUDA_TRY(cudaMemcpy(nw.win_rowptr32, rp.data(), rp.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    if (nnz > 0) {
+      CUDA_TRY(cudaMemcpy(nw.win_col, col.data(), (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice));
+      CUDA_TRY(cudaMemcpy(nw.win_val, val.data(), (size_t)nnz * es, cudaMemcpyHostToDevice));
+    }
+    return B200GF_OK;
+  };
+  if (const int rc = upload_copy()) {
+    free_windows(nw);
+    (void)cudaGetLastError();   // a failed cudaMalloc must not surface at a later launch check
+    return rc;
+  }
+  free_windows(D);
+  D.win_rowptr32 = nw.win_rowptr32; D.win_col = nw.win_col; D.win_val = nw.win_val;
+  D.win_rows = R;
+  D.n_win = (int)W;
+  return B200GF_OK;
+}
+
+// the window copies of a symmetric plan's backward operators alias the forward ones, as the CSR does
+void share_windows(const CsrDev& from, CsrDev& to) {
+  to.win_rows = from.win_rows; to.n_win = from.n_win;
+  to.win_rowptr32 = from.win_rowptr32; to.win_col = from.win_col; to.win_val = from.win_val;
 }
 
 }  // namespace
@@ -209,14 +287,26 @@ int b200gf_plan_create(b200gf_plan** out, int device, int64_t N, int E, const in
     all_sym = all_sym && sym;
     if ((rc = upload(At, N, es, p->fwd[e]))) break;   // forward gathers along columns of S_e
     p->fwd[e].spread = spread;
+    // the default window copy is optional: an operator too large for 32-bit window offsets, or a copy that does not
+    // fit the host or the device, keeps the plain hop
+    const int64_t R = hop_window_rows(N, p->l2_bytes, spread);
+    const auto windows = [&](const HostCsr& M, CsrDev& D) {
+      const int r = R > 0 ? build_windows(M, N, es, R, D) : B200GF_OK;
+      return r == B200GF_EUNSUPPORTED || r == B200GF_ENOMEM ? B200GF_OK : r;
+    };
+    if ((rc = windows(At, p->fwd[e]))) break;
     if (sym) {
       p->bwd[e] = p->fwd[e];
       p->bwd[e].owned = false;
-    } else if ((rc = upload(A, N, es, p->bwd[e]))) break;
+    } else {
+      if ((rc = upload(A, N, es, p->bwd[e]))) break;
+      if ((rc = windows(A, p->bwd[e]))) break;
+    }
     p->bwd[e].spread = spread;
   }
   if (rc) { b200gf_plan_destroy(p); return rc; }
   p->symmetric = all_sym;
+  p->from_gso = true;
   *out = p;
   return B200GF_OK;
 }
@@ -330,8 +420,51 @@ int64_t b200gf_plan_info(const b200gf_plan* plan, int what) {
     case 5: { int64_t s = 0; for (auto& d : plan->fwd) s += d.nnz; return s; }
     case 6: return plan->symmetric ? 1 : 0;
     case 7: return plan->l2_bytes;
+    case 8: return plan->fwd.empty() ? 0 : plan->fwd[0].win_rows;
     default: return B200GF_EINVAL;
   }
+}
+
+int b200gf_plan_set_hop_windows(b200gf_plan* plan, int64_t rows) {
+  if (!plan || rows < 0) return B200GF_EINVAL;
+  if (!plan->from_gso) return B200GF_EUNSUPPORTED;
+  DeviceGuard guard;
+  CUDA_TRY(cudaSetDevice(plan->device));
+  CUDA_TRY(cudaDeviceSynchronize());   // no hop in flight reads the copies about to be replaced
+  const int64_t N = plan->n_rows;
+  const size_t es = dtype_size(plan->dtype);
+  if (rows > 0) {   // sizes no copy can take: the plan stays as it is
+    if (N == 0 || ((N - 1) / rows + 1) * (N + 1) >= (int64_t)INT32_MAX) return B200GF_EUNSUPPORTED;
+    for (int e = 0; e < plan->E; ++e)
+      if (plan->fwd[e].nnz >= (int64_t)INT32_MAX || plan->bwd[e].nnz >= (int64_t)INT32_MAX) return B200GF_EUNSUPPORTED;
+  }
+  // the backward operators of a symmetric plan alias the forward ones and their copies: they are re-pointed after the
+  // forward ones change, so that no operator keeps pointers into a freed copy
+  const auto share_all = [&]() {
+    for (int e = 0; e < plan->E; ++e)
+      if (!plan->bwd[e].owned) share_windows(plan->fwd[e], plan->bwd[e]);
+  };
+  for (int e = 0; e < plan->E; ++e) {
+    for (int dir = 0; dir < 2; ++dir) {
+      CsrDev& D = dir == 0 ? plan->fwd[e] : plan->bwd[e];
+      if (!D.owned) continue;
+      if (rows == 0) { free_windows(D); continue; }
+      HostCsr M;
+      int rc = fetch_csr(M, N, es, D.rowptr, D.col, D.val);
+      if (rc == B200GF_OK) rc = build_windows(M, N, es, rows, D);
+      if (rc) {   // a failed rebuild leaves no copy anywhere: every hop of the plan takes the plain path
+        for (int f = 0; f < plan->E; ++f) {
+          free_windows(plan->fwd[f]);
+          free_windows(plan->bwd[f]);
+        }
+        share_all();
+        return rc;
+      }
+      share_all();
+    }
+  }
+  share_all();
+  return B200GF_OK;
 }
 
 int b200gf_plan_set_l2_bytes(b200gf_plan* plan, int64_t bytes) {

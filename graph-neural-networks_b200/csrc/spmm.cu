@@ -9,6 +9,8 @@
 //     U loads in flight per lane, col/val read once per row and broadcast by SHFL, 48 resident warps per SM,
 //     L2 evict_last policy on the gathered rows;
 //   * narrower rows: several rows per warp (spmm_hop_multirow_kernel);
+//   * operators with a window-major copy (million-node graphs): one launch per (128-byte column chunk, source window),
+//     each adding its window's sums into dst (launch_windows);
 //   * optional epilogue: the computed row slice is also stored over NVLink into a peer's buffer (b200gf_hop_scatter).
 #include <cstdlib>
 #include <cstring>
@@ -22,6 +24,16 @@
 #endif
 #ifndef B200GF_HOP_L2_FRAC
 #define B200GF_HOP_L2_FRAC 1.0f
+#endif
+// geometry and L2 policy of the windowed hop (launch_windows), for tools/hop_window_bench.py's sweep
+#ifndef B200GF_HOP_WIN_GS
+#define B200GF_HOP_WIN_GS 4
+#endif
+#ifndef B200GF_HOP_WIN_U
+#define B200GF_HOP_WIN_U 4
+#endif
+#ifndef B200GF_HOP_WIN_HINT
+#define B200GF_HOP_WIN_HINT 3
 #endif
 
 namespace b200gf {
@@ -182,6 +194,58 @@ static int hop_chunk_lanes(int64_t n_src, int nw, int64_t l2_bytes, bool spread)
   return L0;
 }
 
+// Windowed hop over rows of at least 128 bytes (CsrDev::win_*): one launch per (128-byte column chunk, source window),
+// chunk-major then window-major on the stream, so that the gathers of a launch read one window's rows of one chunk, an
+// L2-sized range.  Window 0 stores its sums, every later window adds its sums into dst (EPI_ACCUM).  Four 32-byte lanes
+// own a row's chunk and a warp works on 32 / GS rows (spmm_hop_multirow_v2_kernel); a window holds few entries per row,
+// so that with GS = 4 a row needs no cross-lane fold.  Written columns: [0, padded(C)), as the plain hop.
+template <typename T, int MODE>
+static int launch_window(int sm_count, const int32_t* rowptr, const CsrDev& A, int64_t n_rows, const T* src,
+                         int64_t src_ld, T* dst, int64_t dst_ld, int C, cudaStream_t st) {
+  constexpr int VEC = 32 / sizeof(T), L = 4, GS = B200GF_HOP_WIN_GS, U = B200GF_HOP_WIN_U, THREADS = 256;
+  constexpr int MINB = sizeof(T) == 4 ? 4 : 3, HINT = B200GF_HOP_WIN_HINT;
+  auto kern = spmm_hop_multirow_v2_kernel<T, int32_t, VEC, L, GS, U, THREADS, MINB, HINT, MODE>;
+  constexpr int rows_per_block = (THREADS / 32) * (32 / GS);
+  int occ = 0;
+  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, 0));
+  if (occ < 1) occ = 1;
+  const int64_t blocks = std::min<int64_t>((n_rows + rows_per_block - 1) / rows_per_block, (int64_t)sm_count * occ);
+  kern<<<(unsigned)blocks, THREADS, 0, st>>>(rowptr, A.win_col, reinterpret_cast<const T*>(A.win_val), src, (int)src_ld,
+                                             dst, (int)dst_ld, (int)n_rows, C, ScatterParam<T, MODE>{});
+  LAUNCH_CHECK();
+  return B200GF_OK;
+}
+
+template <typename T>
+static int launch_windows(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst,
+                          int64_t dst_ld, int C, cudaStream_t st) {
+  if (n_rows == 0) return B200GF_OK;
+  constexpr int CW = 128 / sizeof(T);   // columns per chunk
+  for (int c0 = 0; c0 < C; c0 += CW) {
+    const int Cc = std::min(CW, C - c0);
+    for (int w = 0; w < A.n_win; ++w) {
+      const int32_t* rp = A.win_rowptr32 + (int64_t)w * (n_rows + 1);
+      const int rc = w == 0 ? launch_window<T, EPI_NONE>(sm_count, rp, A, n_rows, src + c0, src_ld, dst + c0, dst_ld, Cc, st)
+                            : launch_window<T, EPI_ACCUM>(sm_count, rp, A, n_rows, src + c0, src_ld, dst + c0, dst_ld, Cc, st);
+      if (rc) return rc;
+    }
+  }
+  return B200GF_OK;
+}
+
+// Rows R per source window of the default window-major operator copy (b200gf_plan_create), 0 for none: only when not
+// even a 128-byte chunk of the source fits the L2 (hop_chunk_lanes has no chunk left to narrow), the gathers spread over
+// the whole source, and the source splits into at most 8 windows.  Windows of 5/8 of the L2 (256 000 rows, 32.8 MB on an
+// H100): 250k-row windows ran the N = 1M, 64-column fp32 hop in 2.43 against 2.56 ms, 200k and 333k rows in 2.47 and
+// 2.44, 125k rows (16 MB) in 2.65.  Every window after the first re-reads and re-writes the destination and the window
+// offsets, so the gain shrinks as windows are added: W = 4 (N = 1M) gained 5 % per hop, W = 8 (N = 2M) 1.4 % (5.67
+// against 5.60 ms); more windows were not measured and are not taken.
+int64_t hop_window_rows(int64_t n_src, int64_t l2_bytes, bool spread) {
+  if (!spread || l2_bytes <= 0 || n_src * 128 <= l2_bytes) return 0;
+  const int64_t R = l2_bytes * 5 / 8 / 128;
+  return R > 0 && n_src <= 8 * R ? R : 0;
+}
+
 template <typename T>
 static int launch_typed(int sm_count, int64_t l2_bytes, const CsrDev& A, int64_t n_rows, const void* src_, int64_t src_ld,
                         void* dst_, int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
@@ -236,6 +300,15 @@ static int launch_typed(int sm_count, int64_t l2_bytes, const CsrDev& A, int64_t
       if (sh && sh->n_peers > 0) return launch_multirow_v2<T, EPI_SCATTER>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
       return launch_multirow_v2<T, EPI_NONE>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, nullptr);
     }
+  }
+  // rows of at least 128 bytes of an operator with a window-major copy: the windowed hop (32-byte aligned rows, 32-bit
+  // offsets), unless the plan's L2 size is 0 or the scatter epilogue is fused
+  if (A.n_win > 0 && nv >= 8 && l2_bytes > 0 && !(sh && sh->n_peers > 0)) {
+    constexpr int VW = 32 / sizeof(T);
+    const int Cw = (C + VW - 1) / VW * VW;
+    if (src_ld % VW == 0 && dst_ld % VW == 0 && Cw <= src_ld && Cw <= dst_ld && (reinterpret_cast<uintptr_t>(src) & 31) == 0 &&
+        (reinterpret_cast<uintptr_t>(dst) & 31) == 0 && src_ld <= INT32_MAX && dst_ld <= INT32_MAX && n_rows <= INT32_MAX)
+      return launch_windows<T>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st);
   }
   if (nv <= 1) return launch_multirow<T, VEC, 1, 8, 1, MB>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
   if (nv <= 2) return launch_multirow<T, VEC, 2, 8, 2, MB>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);

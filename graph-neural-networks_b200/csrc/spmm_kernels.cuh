@@ -101,6 +101,21 @@ __device__ __forceinline__ void store_vec(T* p, const Acc<T, VEC>& a) {
 template <typename V>
 __device__ __forceinline__ V ld_stream(const V* p) { return __ldcs(p); }
 
+// streaming (ld.global.cs) read of a 32-byte lane: two adjacent 16-byte loads
+template <typename T, int VEC>
+__device__ __forceinline__ Acc<T, VEC> load_stream_vec(const T* p) {
+  static_assert(VEC * sizeof(T) == 32, "32-byte lanes only");
+  Acc<T, VEC> a;
+  if constexpr (sizeof(T) == 4) {
+    const float4 lo = __ldcs(reinterpret_cast<const float4*>(p)), hi = __ldcs(reinterpret_cast<const float4*>(p) + 1);
+    a.v[0] = lo.x; a.v[1] = lo.y; a.v[2] = lo.z; a.v[3] = lo.w; a.v[4] = hi.x; a.v[5] = hi.y; a.v[6] = hi.z; a.v[7] = hi.w;
+  } else {
+    const double2 lo = __ldcs(reinterpret_cast<const double2*>(p)), hi = __ldcs(reinterpret_cast<const double2*>(p) + 1);
+    a.v[0] = lo.x; a.v[1] = lo.y; a.v[2] = hi.x; a.v[3] = hi.y;
+  }
+  return a;
+}
+
 constexpr unsigned FULL = 0xffffffffu;
 
 // Fused hop + collective (feature-sharded multi-GPU path): besides the local result row, each computed row slice is
@@ -293,7 +308,8 @@ __device__ __forceinline__ void bcast_store(const BcastArgs<T>& bc, int64_t row,
 // epilogue of the v2 / async kernels.  MODE 0: plain hop; 1: feature-sharded scatter (ScatterArgs); 2: row broadcast.
 //                               3 (2-D process grid): both — the row is all-gathered inside the rank's column group AND its
 //                               slice is delivered to the row's contraction owner inside the rank's row group.
-constexpr int EPI_NONE = 0, EPI_SCATTER = 1, EPI_BCAST = 2, EPI_GRID = 3;
+//                               4: the row slice is added into dst (source windows after the first of a windowed hop).
+constexpr int EPI_NONE = 0, EPI_SCATTER = 1, EPI_BCAST = 2, EPI_GRID = 3, EPI_ACCUM = 4;
 template <typename T, int MODE>
 struct ScatterParam {};
 template <typename T>
@@ -313,6 +329,13 @@ __device__ __forceinline__ void hop_epilogue(const ScatterParam<T, MODE>& sp, T*
     if (sp.a.n_peers > 0) bcast_store<T, VEC>(sp.a, row, cbase, acc);   // n_peers == 0: last hop of a chain, no all-gather
     else if (dst != nullptr) store_vec<T, VEC, SH>(dst + (int64_t)row * dst_ld + cbase, acc);
     scatter_store<T, VEC>(sp.s, row, cbase, acc);
+  } else if constexpr (MODE == EPI_ACCUM) {
+    // dst is read and written once per window: streaming (evict-first) accesses keep the gathered window in the L2
+    T* p = dst + (int64_t)row * dst_ld + cbase;
+    Acc<T, VEC> a = load_stream_vec<T, VEC>(p);
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) a.v[i] += acc.v[i];
+    store_vec<T, VEC, 1>(p, a);
   } else {
     store_vec<T, VEC, SH>(dst + (int64_t)row * dst_ld + cbase, acc);
     if constexpr (MODE == EPI_SCATTER) {
@@ -452,7 +475,9 @@ spmm_hop_multirow_v2_kernel(const IDX* __restrict__ rowptr, const int32_t* __res
 #pragma unroll
       for (int i = 0; i < VEC; ++i) acc.v[i] += __shfl_xor_sync(FULL, acc.v[i], off);
     }
-    if (sub == 0 && col_ok && row_ok) hop_epilogue<T, VEC, SCATTER, 0>(sp, dst, dst_ld, row, cbase, acc);
+    // a row with no entries in a source window after the first leaves its partial sums as they are
+    const bool add_ok = SCATTER != EPI_ACCUM || len > 0;
+    if (sub == 0 && col_ok && row_ok && add_ok) hop_epilogue<T, VEC, SCATTER, 0>(sp, dst, dst_ld, row, cbase, acc);
   }
 }
 

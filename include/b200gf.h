@@ -97,13 +97,28 @@ void b200gf_plan_destroy(b200gf_plan* plan);
 
 /* introspection: what = 0 n_rows, 1 n_cols, 2 E, 3 dtype, 4 device, 5 nnz (sum over e, forward operator),
  * 6 symmetric (1 if every S_e == S_e^T bit-for-bit, so both operators share storage), 7 L2 bytes the hops size their
- * column chunks against (b200gf_plan_set_l2_bytes) */
+ * column chunks against (b200gf_plan_set_l2_bytes), 8 rows R per source window of the window-major operator copies
+ * (b200gf_plan_set_hop_windows), 0 when the plan has none */
 int64_t b200gf_plan_info(const b200gf_plan* plan, int what);
 
 /* L2 size (bytes) the plan's hops size their gathered column chunks against; plan creation reads it from the device
  * (cudaDevAttrL2CacheSize).  0 turns the sizing off: every hop then uses the chunk width its row width alone selects.
  * Results differ only by the summation order of the chunk fold.  For A/B timing and tests; bytes < 0 is EINVAL. */
 int b200gf_plan_set_l2_bytes(b200gf_plan* plan, int64_t bytes);
+
+/* Window-major copies of the plan's gather operators: window w holds the entries whose source row lies in
+ * [w * rows, (w + 1) * rows).  A hop with a plain epilogue over rows of at least 128 bytes then runs one launch per
+ * (128-byte column chunk, window), each adding its window's partial sums into the destination, so that what the
+ * gathers read at a time is an L2-sized source range.  b200gf_plan_create builds them when a 128-byte chunk of the
+ * source does not fit the L2 and the gathers spread over the whole source; the plan's L2 size at 0 turns their use off.
+ * The default takes at most 8 windows.  rows = 0 drops the copies, rows > 0 rebuilds them.  This is a setup call: it
+ * synchronizes the device, frees and allocates, so a CUDA graph captured on the plan before it reads freed copies and
+ * must be captured again.  Results differ from the plain hop only by the summation order of the window sums.
+ * rows < 0 or a null plan is EINVAL; plans from b200gf_plan_create_ops / _create_device are EUNSUPPORTED, and so is a
+ * window count whose offsets W * (N + 1) or operator whose nnz do not fit 32 bits (the plan is left as it was).  Any
+ * other failure of a rebuild (ENOMEM, a CUDA error) leaves the plan without window copies: every hop then takes the
+ * plain path. */
+int b200gf_plan_set_hop_windows(b200gf_plan* plan, int64_t rows);
 
 /* ------------------------------------------------------------------------------------------------
  * LSIGF forward  (graphML.py:83-176)
