@@ -104,9 +104,11 @@ static int launch_multirow(int sm_count, const CsrDev& A, int64_t n_rows, const 
   return B200GF_OK;
 }
 
-// Round-2 kernel (spmm_kernels.cuh: spmm_hop_v2_kernel): 32-byte lanes (two adjacent LDG.128), 32-bit index arithmetic.
-// L lanes x 32 bytes cover a row chunk; 32/L neighbours per warp-wide load, U loads in flight per lane; 4 blocks of 256
-// threads per SM (64 registers); column chunks on blockIdx.y.
+// Round-2 kernel (spmm_kernels.cuh: spmm_hop_v2_kernel): 32-byte lanes loaded as two 16-byte halves, 32-bit index
+// arithmetic.  L lanes x 32 bytes cover a row chunk: the lanes' first halves its first L*16 bytes, their second halves the
+// rest (LaneMap; the NVLink epilogues keep a lane's 32 bytes adjacent), so every LDG.128 / STG.128 of a lane group covers
+// whole 32-byte sectors; 32/L neighbours per warp-wide load, U loads in flight per lane; 4 blocks of 256 threads per SM
+// (64 registers); column chunks on blockIdx.y.
 template <typename T, int L, int SCATTER>
 static int launch_v2(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst, int64_t dst_ld,
                      int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {

@@ -5,9 +5,12 @@
 // Mapping (sm_90a, 132 SMs):
 //   * one warp per (row, column chunk) work item, grid-stride over items in chunk-major order, so that at any
 //     time all resident warps gather from the same column slab (keeps it L2-resident when N * chunk_bytes fits);
-//   * L lanes x 16-byte vectors cover the chunk; the 32/L lane groups each take a different neighbour, so one
-//     warp-wide LDG.128 fetches 32/L whole neighbour rows (every 32-byte sector fully used);
-//   * U independent LDG.128 per lane are in flight before the FMAs (memory-level parallelism);
+//   * L lanes cover the chunk of a neighbour row; the 32/L lane groups each take a different neighbour, so one
+//     warp-wide load fetches 32/L neighbour rows;
+//   * the wide-row kernels (v2) give each lane 32 bytes as two 16-byte halves (sm_90 has no 256-bit load).  The first
+//     halves of a group's L lanes are the chunk's first L*16 bytes and the second halves the rest (LaneMap), so each
+//     warp-wide LDG.128 or STG.128 covers whole 32-byte sectors;
+//   * U independent loads per lane are in flight before the FMAs (memory-level parallelism);
 //   * col/val of a row are read once, coalesced (lane i holds entry i), and broadcast with SHFL;
 //   * PF (template flag, off in the library): prefetch of the next row's col/val and of the rowptr pair after it while
 //     the current row is gathered — it costs registers and issue slots; kept for the sweep tool.
@@ -53,12 +56,6 @@ __device__ __forceinline__ Acc<T, VEC> load_vec(const T* p, uint64_t pol) {
                    : "=f"(t.x), "=f"(t.y), "=f"(t.z), "=f"(t.w) : "l"(p), "l"(pol));
     }
     a.v[0] = t.x; a.v[1] = t.y; a.v[2] = t.z; a.v[3] = t.w;
-  } else if constexpr (VEC * sizeof(T) == 32) {
-    // 32-byte lane: one lane covers a whole 32-byte sector with two adjacent 16-byte loads (sm_90 has no 256-bit load)
-    const Acc<T, VEC / 2> lo = load_vec<T, VEC / 2, HINT>(p, pol);
-    const Acc<T, VEC / 2> hi = load_vec<T, VEC / 2, HINT>(p + VEC / 2, pol);
-#pragma unroll
-    for (int i = 0; i < VEC / 2; ++i) { a.v[i] = lo.v[i]; a.v[VEC / 2 + i] = hi.v[i]; }
   } else if constexpr (VEC == 2) {
     double2 t;
     if constexpr (HINT == 0) {
@@ -101,17 +98,17 @@ __device__ __forceinline__ void store_vec(T* p, const Acc<T, VEC>& a) {
 template <typename V>
 __device__ __forceinline__ V ld_stream(const V* p) { return __ldcs(p); }
 
-// streaming (ld.global.cs) read of a 32-byte lane: two adjacent 16-byte loads
-template <typename T, int VEC>
-__device__ __forceinline__ Acc<T, VEC> load_stream_vec(const T* p) {
-  static_assert(VEC * sizeof(T) == 32, "32-byte lanes only");
-  Acc<T, VEC> a;
+// streaming (ld.global.cs) 16-byte read: one half of a 32-byte lane, or a whole 16-byte lane
+template <typename T, int H>
+__device__ __forceinline__ Acc<T, H> load_stream_16(const T* p) {
+  static_assert(H * sizeof(T) == 16, "16-byte reads only");
+  Acc<T, H> a;
   if constexpr (sizeof(T) == 4) {
-    const float4 lo = __ldcs(reinterpret_cast<const float4*>(p)), hi = __ldcs(reinterpret_cast<const float4*>(p) + 1);
-    a.v[0] = lo.x; a.v[1] = lo.y; a.v[2] = lo.z; a.v[3] = lo.w; a.v[4] = hi.x; a.v[5] = hi.y; a.v[6] = hi.z; a.v[7] = hi.w;
+    const float4 t = __ldcs(reinterpret_cast<const float4*>(p));
+    a.v[0] = t.x; a.v[1] = t.y; a.v[2] = t.z; a.v[3] = t.w;
   } else {
-    const double2 lo = __ldcs(reinterpret_cast<const double2*>(p)), hi = __ldcs(reinterpret_cast<const double2*>(p) + 1);
-    a.v[0] = lo.x; a.v[1] = lo.y; a.v[2] = hi.x; a.v[3] = hi.y;
+    const double2 t = __ldcs(reinterpret_cast<const double2*>(p));
+    a.v[0] = t.x; a.v[1] = t.y;
   }
   return a;
 }
@@ -319,28 +316,92 @@ struct ScatterParam<T, EPI_BCAST> { BcastArgs<T> a; };
 template <typename T>
 struct ScatterParam<T, EPI_GRID> { ScatterArgs<T> s; BcastArgs<T> a; };
 
-// shared epilogue of the v2 kernels
-template <typename T, int VEC, int MODE, int SH>
+// Columns of the two 16-byte halves (H = VEC/2 columns each) of lane cl's 32-byte accumulator in a row chunk of L
+// lanes, relative to the chunk's first column: the first half starts at lo(cl), the second HI columns after it.
+//   SPLIT (the local epilogues, EPI_NONE and EPI_ACCUM): lane cl owns [cl*H, +H) and [L*H + cl*H, +H).  In each of a
+//     lane's two 16-byte loads and stores the L lanes of a group cover L*16 contiguous bytes: whole 32-byte sectors
+//     (whole 128-byte lines for L >= 8);
+//   otherwise (the NVLink epilogues, which store a lane's 32 bytes as one piece): lane cl owns [cl*VEC, +VEC), HI = H.
+// Either way a column is summed by the same lane group over the same neighbours in the same order, so both mappings give
+// bit-identical sums.  A half is live when it starts below the padded width (C rounded up to VEC): columns
+// [0, padded(C)) are written, nothing past them.
+template <int VEC, int L, bool SPLIT>
+struct LaneMap {
+  static constexpr int H = VEC / 2;
+  static constexpr int HI = SPLIT ? L * H : H;
+  __host__ __device__ static constexpr int lo(int cl) { return SPLIT ? cl * H : cl * VEC; }
+};
+template <int MODE>
+constexpr bool split_lanes = MODE == EPI_NONE || MODE == EPI_ACCUM;
+// The v2 kernels take 32-byte lanes (the library) or 16-byte lanes (variants of tools/spmm_sweep.cu).  A 16-byte lane is
+// one load and one store, already whole sectors for every two lanes, so it keeps the adjacent map: lane cl owns
+// [cl*VEC, +VEC).
+template <typename T, int VEC>
+constexpr bool wide_lane = VEC * sizeof(T) == 32;
+template <typename T, int VEC, int L, int MODE>
+using LaneMapOf = LaneMap<VEC, L, wide_lane<T, VEC> && split_lanes<MODE>>;
+
+// a 32-byte lane's two 16-byte halves, at p and p + HI (a half that is not live reads nothing and holds zeros), or a
+// 16-byte lane's one load (when lo_ok)
+template <typename T, int VEC, int HINT, int HI>
+__device__ __forceinline__ Acc<T, VEC> load_lane(const T* p, bool lo_ok, bool hi_ok, uint64_t pol) {
+  static_assert(VEC * sizeof(T) == 16 || VEC * sizeof(T) == 32, "16- or 32-byte lanes only");
+  if constexpr (!wide_lane<T, VEC>) {
+    Acc<T, VEC> a;
+    if (lo_ok) a = load_vec<T, VEC, HINT>(p, pol); else a.zero();
+    return a;
+  }
+  constexpr int H = VEC / 2;
+  Acc<T, H> lo, hi;
+  if (lo_ok) lo = load_vec<T, H, HINT>(p, pol); else lo.zero();
+  if (hi_ok) hi = load_vec<T, H, HINT>(p + HI, pol); else hi.zero();
+  Acc<T, VEC> a;
+#pragma unroll
+  for (int i = 0; i < H; ++i) { a.v[i] = lo.v[i]; a.v[H + i] = hi.v[i]; }
+  return a;
+}
+
+// shared epilogue of the v2 kernels; called for lanes whose first half is live (the peer epilogues: the whole lane)
+template <typename T, int VEC, int L, int MODE, int SH>
 __device__ __forceinline__ void hop_epilogue(const ScatterParam<T, MODE>& sp, T* __restrict__ dst, int dst_ld, int row, int cbase,
-                                             const Acc<T, VEC>& acc) {
+                                             bool hi_ok, const Acc<T, VEC>& acc) {
+  static_assert(VEC * sizeof(T) == 16 || VEC * sizeof(T) == 32, "16- or 32-byte lanes only");
+  constexpr int H = VEC / 2, HI = LaneMapOf<T, VEC, L, MODE>::HI;
   if constexpr (MODE == EPI_BCAST) {
     bcast_store<T, VEC>(sp.a, row, cbase, acc);              // the rank's own copy is one of the destinations
   } else if constexpr (MODE == EPI_GRID) {
     if (sp.a.n_peers > 0) bcast_store<T, VEC>(sp.a, row, cbase, acc);   // n_peers == 0: last hop of a chain, no all-gather
     else if (dst != nullptr) store_vec<T, VEC, SH>(dst + (int64_t)row * dst_ld + cbase, acc);
     scatter_store<T, VEC>(sp.s, row, cbase, acc);
-  } else if constexpr (MODE == EPI_ACCUM) {
-    // dst is read and written once per window: streaming (evict-first) accesses keep the gathered window in the L2
-    T* p = dst + (int64_t)row * dst_ld + cbase;
-    Acc<T, VEC> a = load_stream_vec<T, VEC>(p);
-#pragma unroll
-    for (int i = 0; i < VEC; ++i) a.v[i] += acc.v[i];
-    store_vec<T, VEC, 1>(p, a);
-  } else {
+  } else if constexpr (MODE == EPI_SCATTER) {
     store_vec<T, VEC, SH>(dst + (int64_t)row * dst_ld + cbase, acc);
-    if constexpr (MODE == EPI_SCATTER) {
-      if (sp.a.n_peers > 0) scatter_store<T, VEC>(sp.a, row, cbase, acc);
+    if (sp.a.n_peers > 0) scatter_store<T, VEC>(sp.a, row, cbase, acc);
+  } else if constexpr (!wide_lane<T, VEC>) {
+    // 16-byte lane: one read (EPI_ACCUM) and one store
+    T* p = dst + (int64_t)row * dst_ld + cbase;
+    Acc<T, VEC> a = acc;
+    if constexpr (MODE == EPI_ACCUM) {
+      const Acc<T, VEC> d = load_stream_16<T, VEC>(p);
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) a.v[i] = d.v[i] + a.v[i];
     }
+    store_vec<T, VEC, MODE == EPI_ACCUM ? 1 : SH>(p, a);
+  } else {
+    T* p = dst + (int64_t)row * dst_ld + cbase;
+    Acc<T, H> a0, a1;
+#pragma unroll
+    for (int i = 0; i < H; ++i) { a0.v[i] = acc.v[i]; a1.v[i] = acc.v[H + i]; }
+    if constexpr (MODE == EPI_ACCUM) {
+      // dst is read and written once per window: streaming (evict-first) accesses keep the gathered window in the L2.
+      // Both halves are read before either is written, so that the two reads are in flight together.
+      Acc<T, H> d0 = load_stream_16<T, H>(p), d1;
+      if (hi_ok) d1 = load_stream_16<T, H>(p + HI); else d1.zero();
+#pragma unroll
+      for (int i = 0; i < H; ++i) { a0.v[i] = d0.v[i] + a0.v[i]; a1.v[i] = d1.v[i] + a1.v[i]; }
+    }
+    constexpr int SHs = MODE == EPI_ACCUM ? 1 : SH;
+    store_vec<T, H, SHs>(p, a0);
+    if (hi_ok) store_vec<T, H, SHs>(p + HI, a1);
   }
 }
 
@@ -357,6 +418,7 @@ spmm_hop_v2_kernel(const IDX* __restrict__ rowptr, const int32_t* __restrict__ c
   if constexpr (HINT == 6)
     asm volatile("createpolicy.fractional.L2::evict_last.L2::evict_first.b64 %0, %1;" : "=l"(pol) : "f"(l2_frac));
   constexpr int S = 32 / L;
+  using Map = LaneMapOf<T, VEC, L, SCATTER>;
   const int lane = threadIdx.x & 31;
   const int sub = lane / L;
   const int cl = lane % L;
@@ -364,8 +426,9 @@ spmm_hop_v2_kernel(const IDX* __restrict__ rowptr, const int32_t* __restrict__ c
   {
     // column chunk = blockIdx.y: the block scheduler hands out all CTAs of chunk 0 first, so the resident warps gather
     // from one column slab at a time (chunk-major order) without a chunk loop in the kernel
-    const int cbase = (int)blockIdx.y * (L * VEC) + cl * VEC;
-    const bool col_ok = cbase < C;
+    const int cbase = (int)blockIdx.y * (L * VEC) + Map::lo(cl);
+    const int Cp = (C + VEC - 1) / VEC * VEC;
+    const bool lo_ok = cbase < Cp, hi_ok = cbase + Map::HI < Cp;
     const T* __restrict__ srcc = src + cbase;
     for (int row = warp0; row < n_rows;) {
       IDX p = __ldg(rowptr + row);
@@ -384,7 +447,7 @@ spmm_hop_v2_kernel(const IDX* __restrict__ rowptr, const int32_t* __restrict__ c
           for (int u = 0; u < U; ++u) {
             const int jj = j + u * S + sub;
             const int32_t cc = __shfl_sync(FULL, c, jj & 31);
-            if ((jj < cnt) && col_ok) buf[u] = load_vec<T, VEC, HINT>(srcc + (int64_t)cc * src_ld, pol);
+            if (jj < cnt) buf[u] = load_lane<T, VEC, HINT, Map::HI>(srcc + (int64_t)cc * src_ld, lo_ok, hi_ok, pol);
             else buf[u].zero();
           }
 #pragma unroll
@@ -407,7 +470,7 @@ spmm_hop_v2_kernel(const IDX* __restrict__ rowptr, const int32_t* __restrict__ c
       unsigned ln, gdx;
       asm volatile("mov.u32 %0, %%laneid;" : "=r"(ln));
       asm volatile("mov.u32 %0, %%nctaid.x;" : "=r"(gdx));
-      if (ln < (unsigned)L && cbase < C) hop_epilogue<T, VEC, SCATTER, SH>(sp, dst, dst_ld, row, cbase, acc);
+      if (ln < (unsigned)L && lo_ok) hop_epilogue<T, VEC, L, SCATTER, SH>(sp, dst, dst_ld, row, cbase, hi_ok, acc);
       row += (int)gdx * (THREADS >> 5);
     }
   }
@@ -424,13 +487,15 @@ spmm_hop_multirow_v2_kernel(const IDX* __restrict__ rowptr, const int32_t* __res
   static_assert(GS % L == 0 && GS <= 32 && (GS / L) * U <= GS, "bad multirow geometry");
   constexpr int RPW = 32 / GS;
   constexpr int S = GS / L;
+  using Map = LaneMapOf<T, VEC, L, SCATTER>;
   uint64_t pol = 0;
   if constexpr (HINT >= 2) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
   const int lane = threadIdx.x & 31;
   const int grp = lane / GS, gl = lane % GS;
   const int sub = gl / L, cl = gl % L;
-  const int cbase = cl * VEC;
-  const bool col_ok = cbase < C;
+  const int cbase = Map::lo(cl);
+  const int Cp = (C + VEC - 1) / VEC * VEC;
+  const bool lo_ok = cbase < Cp, hi_ok = cbase + Map::HI < Cp;
   const T* __restrict__ srcc = src + cbase;
   const int n_warps = gridDim.x * (THREADS >> 5);
   for (int row0 = (blockIdx.x * (THREADS >> 5) + (threadIdx.x >> 5)) * RPW; row0 < n_rows; row0 += n_warps * RPW) {
@@ -457,7 +522,7 @@ spmm_hop_multirow_v2_kernel(const IDX* __restrict__ rowptr, const int32_t* __res
         for (int u = 0; u < U; ++u) {
           const int jj = j + u * S + sub;
           const int32_t cc = __shfl_sync(FULL, c, jj, GS);
-          if ((jj < cnt) && col_ok) buf[u] = load_vec<T, VEC, HINT>(srcc + (int64_t)cc * src_ld, pol);
+          if (jj < cnt) buf[u] = load_lane<T, VEC, HINT, Map::HI>(srcc + (int64_t)cc * src_ld, lo_ok, hi_ok, pol);
           else buf[u].zero();
         }
 #pragma unroll
@@ -477,7 +542,7 @@ spmm_hop_multirow_v2_kernel(const IDX* __restrict__ rowptr, const int32_t* __res
     }
     // a row with no entries in a source window after the first leaves its partial sums as they are
     const bool add_ok = SCATTER != EPI_ACCUM || len > 0;
-    if (sub == 0 && col_ok && row_ok && add_ok) hop_epilogue<T, VEC, SCATTER, 0>(sp, dst, dst_ld, row, cbase, acc);
+    if (sub == 0 && lo_ok && row_ok && add_ok) hop_epilogue<T, VEC, L, SCATTER, 0>(sp, dst, dst_ld, row, cbase, hi_ok, acc);
   }
 }
 
