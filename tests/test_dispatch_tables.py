@@ -26,6 +26,7 @@ TABLES = {
     "test_arma_dispatch": ("ARMA_CASES", lambda f: f.startswith("csrc/arma/"), None),
     "test_attention_dispatch": ("ATTENTION_CASES", None, lambda f: f == EGATE),
     "test_spmm_l2_chunks": ("CASES", None, lambda f: f == "csrc/spmm_kernels.cuh"),
+    "test_recurrent_bounds": ("RECURRENT_CASES", None, lambda f: f.startswith("csrc/")),
 }
 
 

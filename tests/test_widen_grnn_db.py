@@ -13,6 +13,8 @@ import pytest
 import torch
 
 import lsigf_oracle as orc
+from host_filters import SparseSlabOps as _SparseSlabOps
+from host_filters import dense_from_csr as _dense_from_csr
 
 GOLD = np.load(os.path.join(os.path.dirname(__file__), "golden", "grnn_db_cases.npz"))
 TAGS = ["ga", "gb", "gc", "gd", "ge", "gf"]
@@ -23,29 +25,6 @@ def _rel(a, b):
     a = np.asarray(a, np.float64)
     b = np.asarray(b, np.float64)
     return np.abs(a - b).max() / max(np.abs(b).max(), 1e-300)
-
-
-def _dense_from_csr(csr, M, dtype):
-    S = torch.zeros(len(csr), M, M, dtype=dtype)
-    for e, (rowptr, col, val) in enumerate(csr):
-        rows = torch.repeat_interleave(torch.arange(M), rowptr[1:] - rowptr[:-1])
-        S[e, rows, col.long()] = val
-    return S
-
-
-class _SparseSlabOps:
-    """CPU stand-in for delayed._SlabOps: the same per-(t, e) gather operators (slab_csr's `fwd`), applied by torch.sparse
-    (differentiable w.r.t. the dense operand, so the recursion's autograd wiring is exercised too)."""
-
-    def __init__(self, S):
-        from gnn_b200 import delayed
-        fwd, _, R = delayed.slab_csr(S)
-        self.hops = 0
-        self.A = [torch.sparse_csr_tensor(rp, col.long(), val, size=(R, R)).to_sparse_coo() for (rp, col, val) in fwd]
-
-    def hop(self, o, src):
-        self.hops += 1
-        return torch.sparse.mm(self.A[o], src)
 
 
 @pytest.fixture
