@@ -144,7 +144,12 @@ static int launch_v2_sc(int sm_count, const CsrDev& A, int64_t n_rows, const T* 
                         int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
   if (bh && sh) return launch_v2<T, L, EPI_GRID>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
   if (bh) return launch_v2<T, L, EPI_BCAST>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, nullptr, bh);
-  if (sh && sh->n_peers > 0) return launch_v2<T, L, EPI_SCATTER>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
+  if (sh && sh->n_peers > 0) {
+    // the feature-sharded scatter sizes its chunks by row width alone (hop_chunk_lanes without an L2 budget), so L >= 8:
+    // no 4-lane scatter kernel is compiled
+    if constexpr (L >= 8) return launch_v2<T, L, EPI_SCATTER>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
+    else return B200GF_EUNSUPPORTED;
+  }
   return launch_v2<T, L, EPI_NONE>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, nullptr, nullptr);
 }
 
@@ -367,6 +372,8 @@ int launch_bcast_rows(int dtype, const void* src, int64_t src_ld, int64_t n_rows
   if (n_rows == 0) return B200GF_OK;
   const int blocks = 132 * 8;
   if ((reinterpret_cast<uintptr_t>(src) & 15) || (reinterpret_cast<uintptr_t>(bh->mc) & 15)) return B200GF_EUNSUPPORTED;
+  for (int i = 0; i < bh->n_peers; ++i)   // 16-byte vector stores into every peer
+    if (reinterpret_cast<uintptr_t>(bh->peer[i]) & 15) return B200GF_EUNSUPPORTED;
   if (dtype == B200GF_F32) {
     if (C % 4 || src_ld % 4 || bh->out_ld % 4) return B200GF_EUNSUPPORTED;
     bcast_rows_kernel<float, 4><<<blocks, 256, 0, st>>>((const float*)src, src_ld, n_rows, C, make_bcast<float>(bh));
@@ -399,6 +406,7 @@ int launch_scatter_rows(int dtype, const void* src, int64_t src_ld, int64_t n_ro
   if (!src || !sh || sh->n_peers <= 0 || sh->n_peers > MAX_PEERS || C <= 0 || src_ld < C) return B200GF_EINVAL;
   if (n_rows == 0) return B200GF_OK;
   const int blocks = 132 * 8;
+  if (reinterpret_cast<uintptr_t>(src) & 15) return B200GF_EUNSUPPORTED;   // 16-byte vector loads
   if (dtype == B200GF_F32) {
     if (C % 4 || src_ld % 4 || sh->gl % 4 || sh->out_ld % 4 || sh->out_col % 4 || sh->stride_b % 4) return B200GF_EUNSUPPORTED;
     scatter_rows_kernel<float, 4><<<blocks, 256, 0, st>>>((const float*)src, src_ld, n_rows, C, make_scatter<float>(sh));

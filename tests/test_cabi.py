@@ -263,97 +263,6 @@ def test_header_is_plain_c(tmp_path):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
-@pytest.mark.parametrize("C", [40, 64, 320])
-def test_fused_allgather_epilogue_on_one_gpu(C, dtype):
-    """b200gf_hop_bcast / b200gf_bcast_rows (node-sharded multi-GPU path, SURVEY.md §8e) exercised on ONE GPU: the "peers"
-    are just device pointers, so three full-height buffers on the same device stand in for three ranks.  Two row blocks
-    of S^T are computed by two plans (the way two ranks would) and every destination must end up with the complete
-    product; then the peer-flag fence with a single participant must pass."""
-    import ctypes
-    import scipy.sparse as sp
-    import gnn_b200
-    from gnn_b200.gso import Plan
-    from gnn_b200.distributed import row_slice, transpose_csr
-    cabi = gnn_b200._cabi
-    lib = cabi.load()
-    N, R = 900, 450
-    rs = np.random.RandomState(C)
-    m = sp.random(N, N, density=0.03, format="csr", random_state=rs)
-    m.sort_indices()
-    npd = np.float32 if dtype == torch.float32 else np.float64
-    csr = (m.indptr.astype(np.int64), m.indices.astype(np.int32), m.data.astype(npd))
-    st_csr = transpose_csr(csr, N)
-    ld = gnn_b200.padded_ld(C, dtype)
-    X = torch.randn(N, C, dtype=dtype, device="cuda")
-    src = torch.zeros(N, ld, dtype=dtype, device="cuda"); src[:, :C] = X
-    dsts = [torch.full((N, ld), float("nan"), dtype=dtype, device="cuda") for _ in range(3)]
-    peers = cabi.ptr_array([d.data_ptr() for d in dsts])
-    stream = torch.cuda.current_stream().cuda_stream
-    for p in range(2):                                           # "rank" p owns rows [p*R, (p+1)*R)
-        plan = Plan.from_ops([row_slice(st_csr, p * R, (p + 1) * R)], [row_slice(csr, p * R, (p + 1) * R)], R, N, dtype, "cuda")
-        rc = lib.b200gf_hop_bcast(plan.handle, 0, cabi.HOP_FWD, src.data_ptr(), ld, C, peers, 3, None, p * R, ld, stream)
-        assert rc == 0, lib.b200gf_strerror(rc)
-    mr = sp.csr_matrix((m.data.astype(npd).astype(np.float64), m.indices, m.indptr), shape=m.shape)
-    ref = mr.T @ X.double().cpu().numpy()
-    tol = 1e-5 if dtype == torch.float32 else 1e-13
-    for d in dsts:
-        assert _rel(d[:, :C].cpu().numpy(), ref) < tol
-    # all-gather of an existing row block (the k = 0 term)
-    for d in dsts:
-        d.fill_(float("nan"))
-    for p in range(2):
-        blk = src[p * R:(p + 1) * R]
-        rc = lib.b200gf_bcast_rows(cabi.F32 if dtype == torch.float32 else cabi.F64, blk.data_ptr(), ld, R, C, peers, 3, None,
-                                   p * R, ld, stream)
-        assert rc == 0, lib.b200gf_strerror(rc)
-    for d in dsts:
-        assert torch.equal(d[:, :C], X)
-    # peer-flag fence, one participant: signal then wait must return (and count monotonically)
-    flags = torch.zeros(32, dtype=torch.int64, device="cuda")    # [16 flags][step counter ...]
-    for step in (1, 2, 3):
-        assert lib.b200gf_peer_signal(cabi.ptr_array([flags.data_ptr()]), 1, 0, ctypes.c_void_p(flags.data_ptr() + 128), stream) == 0
-        assert lib.b200gf_peer_wait(ctypes.c_void_p(flags.data_ptr()), 1, ctypes.c_void_p(flags.data_ptr() + 128), stream) == 0
-        torch.cuda.synchronize()
-        assert int(flags[0]) == step and int(flags[16]) == step
-
-
-@pytest.mark.gpu
-def test_fused_scatter_epilogue_on_one_gpu():
-    """b200gf_hop_scatter (feature-sharded path) on ONE GPU: two local buffers stand in for the row-owning ranks; every
-    computed row slice must land at [owner, local row, b*stride_b + out_col + g].  C = 16 takes the 32-byte-lane multi-row
-    kernel, C = 8 the 16-byte one, C = 48 the wide single-row kernel."""
-    import scipy.sparse as sp
-    import gnn_b200
-    cabi = gnn_b200._cabi
-    lib = cabi.load()
-    N, R, B, T, G = 1000, 500, 2, 3, 48                           # operand rows [R, B*T*G]; this "rank" owns Gl columns of G
-    m = sp.random(N, N, density=0.02, format="csr", random_state=3)
-    gso = gnn_b200.SparseGSO.from_scipy([m], dtype=torch.float32)
-    plan = gso.plan("cuda")
-    stream = torch.cuda.current_stream().cuda_stream
-    for Gl, g0 in ((8, 8), (4, 16), (24, 24)):
-        Cl = B * Gl
-        ld = gnn_b200.padded_ld(Cl, torch.float32)
-        X = torch.randn(N, Cl, device="cuda")
-        src = torch.zeros(N, ld, device="cuda"); src[:, :Cl] = X
-        dst = torch.empty(N, ld, device="cuda")
-        row_elems = B * T * G
-        ops = [torch.zeros(R, row_elems, device="cuda") for _ in range(2)]
-        t = 1
-        rc = lib.b200gf_hop_scatter(plan.handle, 0, cabi.HOP_FWD, src.data_ptr(), ld, dst.data_ptr(), ld, Cl,
-                                    cabi.ptr_array([o.data_ptr() for o in ops]), 2, R, row_elems, t * G + g0, Gl, T * G, stream)
-        assert rc == 0, lib.b200gf_strerror(rc)
-        ref = torch.tensor(m.T.astype(np.float32).astype(np.float64) @ X.double().cpu().numpy()).float()
-        assert _rel(dst[:, :Cl].cpu().numpy(), ref.numpy()) < 1e-5
-        full = torch.cat(ops).view(N, B, T, G)[:, :, t, g0:g0 + Gl].reshape(N, Cl)
-        assert torch.equal(full, dst[:, :Cl])
-        untouched = torch.cat(ops).view(N, B, T, G).clone()
-        untouched[:, :, t, g0:g0 + Gl] = 0
-        assert float(untouched.abs().max()) == 0.0
-
-
-@pytest.mark.gpu
 def test_launch_counter_counts_library_kernels():
     import gnn_b200
     from gnn_b200 import graphs
@@ -366,59 +275,3 @@ def test_launch_counter_counts_library_kernels():
     gnn_b200.LSIGF(h, gso, x, None)
     # transpose to node-major, 3 hops, tap packing, contraction
     assert lib.b200gf_launch_count(0) == 6 and lib.b200gf_launch_count(1) == 6 and lib.b200gf_launch_count(0) == 0
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
-@pytest.mark.parametrize("Gl", [8, 16, 40])
-def test_grid_epilogue_on_one_gpu(Gl, dtype):
-    """b200gf_hop_grid (2-D process grid) on ONE GPU with local buffers as the peers: rows of one row group, columns of one
-    column group; every row must land (a) in all all-gather destinations at row0 + r and (b) in the contraction operand of
-    its owner at [r % rows_per_peer, b*stride_b + out_col + g]; n_bc = 0 (last hop) must only scatter.
-    Gl*B*4 bytes = 64 (multi-row kernel), 128 (L = 4) and 320 (L = 16) byte rows in fp32."""
-    import scipy.sparse as sp
-    import gnn_b200
-    from gnn_b200.gso import Plan
-    from gnn_b200.distributed import row_slice, transpose_csr
-    cabi = gnn_b200._cabi
-    lib = cabi.load()
-    if dtype == torch.float64 and Gl == 8:
-        Gl = 12                                                     # keep fp64 rows at >= 64 bytes and 32-byte lanes whole
-    N, Rr, Rc, B, T, G = 1200, 600, 200, 2, 3, 3 * Gl               # 2 row groups, 3 owners per row group
-    m = sp.random(N, N, density=0.02, format="csr", random_state=Gl)
-    m.sort_indices()
-    npd = np.float32 if dtype == torch.float32 else np.float64
-    csr = (m.indptr.astype(np.int64), m.indices.astype(np.int32), m.data.astype(npd))
-    st_csr = transpose_csr(csr, N)
-    Cl = B * Gl
-    ld = gnn_b200.padded_ld(Cl, dtype)
-    X = torch.randn(N, Cl, dtype=dtype, device="cuda")
-    src = torch.zeros(N, ld, dtype=dtype, device="cuda"); src[:, :Cl] = X
-    mr = sp.csr_matrix((m.data.astype(npd).astype(np.float64), m.indices, m.indptr), shape=m.shape)
-    ref = torch.tensor(mr.T @ X.double().cpu().numpy())
-    tol = 1e-5 if dtype == torch.float32 else 1e-13
-    stream = torch.cuda.current_stream().cuda_stream
-    row_elems = B * T * G
-    t, g0 = 2, Gl                                                    # term 2, second column group
-    for rg in range(2):
-        plan = Plan.from_ops([row_slice(st_csr, rg * Rr, (rg + 1) * Rr)], None, Rr, N, dtype, "cuda")
-        for n_bc in (2, 0):
-            gathers = [torch.full((N, ld), float("nan"), dtype=dtype, device="cuda") for _ in range(2)]
-            ops = [torch.zeros(Rc, row_elems, dtype=dtype, device="cuda") for _ in range(3)]
-            rc = lib.b200gf_hop_grid(plan.handle, 0, cabi.HOP_FWD, src.data_ptr(), ld, Cl,
-                                     cabi.ptr_array([g.data_ptr() for g in gathers]) if n_bc else None, n_bc, rg * Rr, ld,
-                                     cabi.ptr_array([o.data_ptr() for o in ops]), 3, Rc, row_elems, t * G + g0, Gl, T * G, stream)
-            assert rc == 0, lib.b200gf_strerror(rc)
-            want = ref[rg * Rr:(rg + 1) * Rr]
-            got = torch.cat(ops).view(Rr, B, T, G)[:, :, t, g0:g0 + Gl].reshape(Rr, Cl)
-            assert _rel(got.cpu().numpy(), want.numpy()) < tol
-            rest = torch.cat(ops).view(Rr, B, T, G).clone()
-            rest[:, :, t, g0:g0 + Gl] = 0
-            assert float(rest.abs().max()) == 0.0
-            for gth in gathers:
-                if n_bc:
-                    assert _rel(gth[rg * Rr:(rg + 1) * Rr, :Cl].cpu().numpy(), want.numpy()) < tol
-                    other = torch.cat((gth[:rg * Rr], gth[(rg + 1) * Rr:]))
-                    assert bool(torch.isnan(other).all())                        # only this row group's rows were written
-                else:
-                    assert bool(torch.isnan(gth).all())

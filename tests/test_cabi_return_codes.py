@@ -6,7 +6,9 @@ fails, so it comes back as a CUDA error code (rc <= B200GF_ECUDA).  For the same
 when a CUDA device is visible: placeholder pointers must never reach a kernel.
 
 The plan-based entry points need a plan, and b200gf_plan_create needs a device.  A small helper compiled against
-csrc/common.cuh builds host-only plans (no CSR on the device) that get exactly as far as the argument checks need."""
+csrc/common.cuh builds host-only plans (no CSR on the device) that get exactly as far as the argument checks need; a
+plan with v2=1 also carries a placeholder for the 32-bit row offsets, which the fused all-gather and grid epilogues
+require before they launch."""
 import ctypes
 import os
 import shutil
@@ -27,14 +29,16 @@ F32, F64, FM, NM = 0, 1, 0, 1
 P = 0x10000                     # placeholder device pointer (256-byte aligned)
 WS = 0x20000                    # placeholder workspace
 MISALIGNED = 0x101
+RP32 = 0x30000                  # placeholder 32-bit row offsets of a host-only plan
 BIG = 1 << 31                   # > INT32_MAX
 
 _HELPER = r"""
 #include "common.cuh"
-extern "C" b200gf_plan* rc_test_plan(int64_t n_rows, int64_t n_cols, int E, int dtype, int has_bwd) {
+extern "C" b200gf_plan* rc_test_plan(int64_t n_rows, int64_t n_cols, int E, int dtype, int has_bwd, void* rowptr32) {
   b200gf_plan* p = new b200gf_plan();
   p->dtype = dtype; p->n_rows = n_rows; p->n_cols = n_cols; p->E = E; p->has_bwd = has_bwd != 0;
   p->fwd.resize(E); p->bwd.resize(E);
+  for (int e = 0; e < E; ++e) p->fwd[e].rowptr32 = p->bwd[e].rowptr32 = (int32_t*)rowptr32;
   return p;
 }
 extern "C" void rc_test_plan_free(b200gf_plan* p) { delete p; }
@@ -60,14 +64,14 @@ def plans(tmp_path_factory):
     assert out.returncode == 0, out.stdout + out.stderr
     h = ctypes.CDLL(str(so))
     h.rc_test_plan.restype = ctypes.c_void_p
-    h.rc_test_plan.argtypes = [ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int]
+    h.rc_test_plan.argtypes = [ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     h.rc_test_plan_free.argtypes = [ctypes.c_void_p]
     made = {}
 
-    def plan(N=64, E=2, dtype=F32, has_bwd=1, n_cols=None):
-        key = (N, E, dtype, has_bwd, n_cols)
+    def plan(N=64, E=2, dtype=F32, has_bwd=1, n_cols=None, v2=0):
+        key = (N, E, dtype, has_bwd, n_cols, v2)
         if key not in made:
-            made[key] = h.rc_test_plan(N, N if n_cols is None else n_cols, E, dtype, has_bwd)
+            made[key] = h.rc_test_plan(N, N if n_cols is None else n_cols, E, dtype, has_bwd, RP32 if v2 else None)
         return made[key]
 
     yield plan
@@ -86,9 +90,10 @@ def _check(fn, defaults, cases):
     return bad
 
 
-def _ptrs(n, null_at=None):
+def _ptrs(n, null_at=None, shift_at=None, by=0):
+    """n placeholder device pointers, 256-byte aligned; the one at null_at null, the one at shift_at moved by `by` bytes."""
     import gnn_b200
-    return gnn_b200._cabi.ptr_array([0 if i == null_at else P + 0x1000 * i for i in range(n)])
+    return gnn_b200._cabi.ptr_array([0 if i == null_at else P + 0x1000 * i + (by if i == shift_at else 0) for i in range(n)])
 
 
 def _lds(n, ld):
@@ -163,6 +168,127 @@ def _hop(lib, plans):
         (dict(plan=plans(has_bwd=0), direction=0), PASS),
     ]
     return lib.b200gf_hop, d, cases
+
+
+# ------------------------------------------------------------------------------------------------ peer epilogues
+# The fused multi-GPU hops and row copies: ScatterArgs (peer r // rows_per_peer, column b*stride_b + out_col + g of
+# b*gl + g) and BcastArgs (full-height peer buffers, rows from row0).  Scatter peers must be 16-byte aligned (EINVAL);
+# the all-gather and grid epilogues need 32-byte lanes, so their misaligned buffers are EUNSUPPORTED, as is a 16-byte
+# row copy whose source or peer is not 16-byte aligned.
+def _hop_scatter(lib, plans):
+    d = dict(plan=plans(), e=1, direction=1, src=P, src_ld=16, dst=P, dst_ld=16, C=16, peers=_ptrs(2), n_peers=2,
+             rows_per_peer=32, out_ld=96, out_col=8, gl=8, stride_b=48, stream=None)
+    cases = [
+        ({}, PASS), (dict(direction=0), PASS), (dict(plan=plans(v2=1)), PASS), (dict(C=48, src_ld=48, dst_ld=48), PASS),
+        (dict(peers=_ptrs(16), n_peers=16, rows_per_peer=4), PASS), (dict(gl=4, out_col=4), PASS),
+        (dict(plan=None), EINVAL), (dict(src=None), EINVAL), (dict(dst=None), EINVAL), (dict(e=2), EINVAL),
+        (dict(direction=2), EINVAL), (dict(plan=plans(has_bwd=0)), EINVAL),
+        (dict(peers=None), EINVAL), (dict(n_peers=0), EINVAL), (dict(peers=_ptrs(17), n_peers=17), EINVAL),
+        (dict(peers=_ptrs(2, null_at=1)), EINVAL), (dict(rows_per_peer=0), EINVAL), (dict(gl=0), EINVAL),
+        (dict(rows_per_peer=31), EINVAL),                               # 2 x 31 < 64 rows
+        (dict(C=12, src_ld=12, dst_ld=12), EINVAL),                     # C % gl
+        (dict(peers=_ptrs(2, shift_at=1, by=8)), EINVAL),               # peer not 16-byte aligned
+        (dict(C=0), EINVAL), (dict(src_ld=15), EINVAL), (dict(dst_ld=15), EINVAL),
+        (dict(src=P + 8), EUNSUPPORTED), (dict(src_ld=18), EUNSUPPORTED), (dict(out_col=2), EUNSUPPORTED),
+        (dict(stride_b=50), EUNSUPPORTED), (dict(out_ld=98), EUNSUPPORTED),
+        # order: the peers, then rows and C % gl, then the hop's own checks
+        (dict(plan=None, peers=None), EINVAL), (dict(peers=_ptrs(17), n_peers=17, src=P + 8), EINVAL),
+        (dict(rows_per_peer=31, src=P + 8), EINVAL), (dict(C=12, out_col=2), EINVAL),
+    ]
+    return lib.b200gf_hop_scatter, d, cases
+
+
+def _hop_bcast(lib, plans):
+    d = dict(plan=plans(v2=1), e=1, direction=1, src=P, src_ld=48, C=48, peers=_ptrs(3), n_peers=3, mc=None, row0=0,
+             out_ld=48, stream=None)
+    cases = [
+        ({}, PASS), (dict(direction=0), PASS), (dict(C=44), PASS), (dict(peers=_ptrs(16), n_peers=16), PASS),
+        (dict(mc=P), PASS), (dict(row0=64, out_ld=56), PASS), (dict(C=24, src_ld=24, out_ld=24), PASS),
+        (dict(plan=None), EINVAL), (dict(src=None), EINVAL), (dict(e=2), EINVAL), (dict(direction=2), EINVAL),
+        (dict(plan=plans(has_bwd=0, v2=1)), EINVAL),
+        (dict(peers=None), EINVAL), (dict(n_peers=0), EINVAL), (dict(peers=_ptrs(17), n_peers=17), EINVAL),
+        (dict(peers=_ptrs(3, null_at=2)), EINVAL), (dict(row0=-1), EINVAL), (dict(out_ld=0), EINVAL),
+        (dict(out_ld=47), EINVAL), (dict(C=0), EINVAL), (dict(src_ld=47), EINVAL),
+        (dict(peers=_ptrs(3, shift_at=1, by=16)), EUNSUPPORTED),        # 16- but not 32-byte aligned peer
+        (dict(peers=_ptrs(3, shift_at=0, by=4)), EUNSUPPORTED),
+        (dict(src=P + 16), EUNSUPPORTED), (dict(mc=P + 16), EUNSUPPORTED), (dict(src_ld=52), EUNSUPPORTED),
+        (dict(out_ld=52), EUNSUPPORTED), (dict(plan=plans()), EUNSUPPORTED),   # no 32-bit offsets
+        (dict(C=16, src_ld=16, out_ld=16), EUNSUPPORTED),               # a 64-byte row: only the grid epilogue has one
+        (dict(C=8, src_ld=8, out_ld=8), EUNSUPPORTED),                  # a 32-byte row
+        # order
+        (dict(peers=None, C=16), EINVAL), (dict(row0=-1, src=P + 16), EINVAL), (dict(out_ld=47, src=P + 16), EINVAL),
+    ]
+    return lib.b200gf_hop_bcast, d, cases
+
+
+def _hop_grid(lib, plans):
+    d = dict(plan=plans(v2=1), e=1, direction=1, src=P, src_ld=16, C=16, bc_peers=_ptrs(2), n_bc=2, row0=0, bc_ld=16,
+             sc_peers=_ptrs(2), n_sc=2, rows_per_peer=32, out_ld=96, out_col=8, gl=8, stride_b=48, stream=None)
+    cases = [
+        ({}, PASS), (dict(direction=0), PASS), (dict(C=48, src_ld=48, bc_ld=48), PASS),
+        (dict(C=24, src_ld=24, bc_ld=24), PASS), (dict(bc_peers=None, n_bc=0), PASS),   # last hop: scatter only
+        (dict(bc_peers=_ptrs(16), n_bc=16, sc_peers=_ptrs(16), n_sc=16, rows_per_peer=4), PASS),
+        (dict(sc_peers=_ptrs(2, shift_at=1, by=16)), PASS),             # scatter peers need 16 bytes only
+        (dict(plan=None), EINVAL), (dict(src=None), EINVAL), (dict(e=2), EINVAL), (dict(direction=2), EINVAL),
+        (dict(plan=plans(has_bwd=0, v2=1)), EINVAL),
+        (dict(bc_peers=None), EINVAL), (dict(bc_peers=_ptrs(17), n_bc=17), EINVAL),
+        (dict(bc_peers=_ptrs(2, null_at=0)), EINVAL), (dict(row0=-1), EINVAL), (dict(bc_ld=0), EINVAL),
+        (dict(bc_peers=None, n_bc=0, sc_peers=None, n_sc=0), EINVAL),   # neither all-gather nor scatter
+        (dict(sc_peers=None), EINVAL), (dict(n_sc=0), EINVAL), (dict(sc_peers=_ptrs(17), n_sc=17), EINVAL),
+        (dict(sc_peers=_ptrs(2, null_at=1)), EINVAL), (dict(sc_peers=_ptrs(2, shift_at=0, by=8)), EINVAL),
+        (dict(rows_per_peer=31), EINVAL), (dict(C=20, src_ld=24, bc_ld=24), EINVAL), (dict(gl=0), EINVAL),
+        (dict(bc_ld=15), EINVAL), (dict(src_ld=15), EINVAL),
+        (dict(bc_peers=_ptrs(2, shift_at=1, by=16)), EUNSUPPORTED), (dict(src=P + 16), EUNSUPPORTED),
+        (dict(out_col=4, gl=4, C=16), EUNSUPPORTED), (dict(out_col=4), EUNSUPPORTED), (dict(stride_b=52), EUNSUPPORTED),
+        (dict(bc_ld=20), EUNSUPPORTED), (dict(plan=plans()), EUNSUPPORTED), (dict(C=8, gl=8, src_ld=8, bc_ld=8), EUNSUPPORTED),
+        # order: all-gather peers, scatter peers, rows and C % gl, then the kernel's alignment
+        (dict(bc_peers=None, sc_peers=None), EINVAL), (dict(n_sc=0, rows_per_peer=31), EINVAL),
+        (dict(rows_per_peer=31, src=P + 16), EINVAL),
+    ]
+    return lib.b200gf_hop_grid, d, cases
+
+
+def _bcast_rows(lib, plans):
+    d = dict(dtype=F32, src=P, src_ld=8, n_rows=N, C=8, peers=_ptrs(2), n_peers=2, mc=None, row0=0, out_ld=8,
+             stream=None)
+    cases = [
+        ({}, PASS), (dict(dtype=F64), PASS), (dict(mc=P), PASS), (dict(C=4, src_ld=12, out_ld=4, row0=5), PASS),
+        (dict(peers=_ptrs(16), n_peers=16), PASS), (dict(peers=_ptrs(2, shift_at=1, by=16)), PASS), (dict(n_rows=0), OK),
+        (dict(src=None), EINVAL), (dict(peers=None), EINVAL), (dict(n_peers=0), EINVAL),
+        (dict(peers=_ptrs(17), n_peers=17), EINVAL), (dict(peers=_ptrs(2, null_at=1)), EINVAL), (dict(row0=-1), EINVAL),
+        (dict(out_ld=0), EINVAL), (dict(out_ld=7), EINVAL), (dict(C=0), EINVAL), (dict(src_ld=7), EINVAL),
+        (dict(peers=_ptrs(2, shift_at=1, by=4)), EUNSUPPORTED),         # every peer takes 16-byte stores
+        (dict(dtype=F64, peers=_ptrs(2, shift_at=0, by=8)), EUNSUPPORTED),
+        (dict(src=P + 8), EUNSUPPORTED), (dict(mc=P + 8), EUNSUPPORTED), (dict(C=6, src_ld=8), EUNSUPPORTED),
+        (dict(dtype=F64, C=5), EUNSUPPORTED), (dict(src_ld=10), EUNSUPPORTED), (dict(out_ld=10), EUNSUPPORTED),
+        (dict(dtype=7), EUNSUPPORTED),
+        # order: an empty copy returns before the alignment and dtype checks
+        (dict(n_rows=0, peers=_ptrs(2, shift_at=1, by=4)), OK), (dict(n_rows=0, dtype=7), OK),
+        (dict(peers=_ptrs(2, null_at=0), src=P + 8), EINVAL), (dict(out_ld=7, peers=_ptrs(2, shift_at=1, by=4)), EINVAL),
+    ]
+    return lib.b200gf_bcast_rows, d, cases
+
+
+def _scatter_rows(lib, plans):
+    d = dict(dtype=F32, src=P, src_ld=16, n_rows=N, C=16, peers=_ptrs(2), n_peers=2, rows_per_peer=32, out_ld=96,
+             out_col=8, gl=8, stride_b=48, stream=None)
+    cases = [
+        ({}, PASS), (dict(dtype=F64), PASS), (dict(gl=4, C=12, out_col=4), PASS),
+        (dict(peers=_ptrs(16), n_peers=16, rows_per_peer=4), PASS), (dict(dtype=F64, src=P + 16), PASS),
+        (dict(n_rows=0), OK),
+        (dict(src=None), EINVAL), (dict(peers=None), EINVAL), (dict(n_peers=0), EINVAL),
+        (dict(peers=_ptrs(17), n_peers=17), EINVAL), (dict(peers=_ptrs(2, null_at=1)), EINVAL),
+        (dict(peers=_ptrs(2, shift_at=1, by=8)), EINVAL), (dict(rows_per_peer=0), EINVAL), (dict(gl=0), EINVAL),
+        (dict(rows_per_peer=31), EINVAL), (dict(C=12), EINVAL), (dict(C=0), EINVAL), (dict(src_ld=15), EINVAL),
+        (dict(src=P + 8), EUNSUPPORTED),                                # 16-byte vector loads of the source
+        (dict(dtype=F64, src=P + 8), EUNSUPPORTED), (dict(src=P + 4), EUNSUPPORTED),
+        (dict(out_col=2), EUNSUPPORTED), (dict(src_ld=18), EUNSUPPORTED), (dict(stride_b=50), EUNSUPPORTED),
+        (dict(out_ld=98), EUNSUPPORTED), (dict(dtype=F64, out_col=1), EUNSUPPORTED), (dict(dtype=7), EUNSUPPORTED),
+        # order
+        (dict(n_rows=0, src=P + 8), OK), (dict(n_rows=0, dtype=7), OK), (dict(src=P + 8, C=12), EINVAL),
+        (dict(rows_per_peer=31, src=P + 8), EINVAL), (dict(peers=_ptrs(2, shift_at=1, by=8), src=P + 8), EINVAL),
+    ]
+    return lib.b200gf_scatter_rows, d, cases
 
 
 M = 4
@@ -467,7 +593,7 @@ def _tap_grad(lib, plans):
 
 ENTRY_POINTS = {f.__name__[1:]: f for f in (
     _lsigf_forward, _lsigf_forward_act, _lsigf_backward, _hop, _nv_forward, _nv_backward, _nv_pack_taps,
-    _arma_forward, _arma_backward, _egate_attention_forward, _egate_attention_backward, _attention_forward,
+    _hop_scatter, _hop_bcast, _hop_grid, _bcast_rows, _scatter_rows, _arma_forward, _arma_backward, _egate_attention_forward, _egate_attention_backward, _attention_forward,
     _attention_backward, _gated_hop_forward, _gated_hop_backward, _ev_forward, _ev_backward, _relu_backward,
     _maxpool_forward, _maxpool_backward, _to_node_major, _to_feature_major, _pack_taps, _tap_contract, _tap_grad)}
 

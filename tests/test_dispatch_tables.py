@@ -27,6 +27,7 @@ TABLES = {
     "test_attention_dispatch": ("ATTENTION_CASES", None, lambda f: f == EGATE),
     "test_spmm_l2_chunks": ("CASES", None, lambda f: f == "csrc/spmm_kernels.cuh"),
     "test_recurrent_bounds": ("RECURRENT_CASES", None, lambda f: f.startswith("csrc/")),
+    "test_peer_epilogues": ("PEER_CASES", None, lambda f: f in ("csrc/spmm.cu", "csrc/spmm_kernels.cuh")),
 }
 
 

@@ -4,7 +4,9 @@ CPU: world_size-2 gloo runs with an oracle-backed `ops` (scipy / numpy stand-ins
 exercises the partitioning, padding, in-place all-gather and reduce-scatter choreography against the fp64 oracle.
 GPU (-m gpu, needs >= 2 devices): the same through NCCL and the CUDA building blocks."""
 import os
+import pickle
 import socket
+import tempfile
 
 import numpy as np
 import pytest
@@ -80,115 +82,164 @@ def _case(N=203, B=2, G=6, F=8, K=4, E=2, seed=3):
     return mats, x, h, b
 
 
-def _worker(rank, world, port, backend, mode, dtype_name, result_q, G=6, backward=True, F=8, grid=None, K=4):
-    import gnn_b200
-    from gnn_b200.distributed import PartitionedLSIGF
+def _worker(rank, world, port, backend, runs, out_path):
+    """One rank: joins the process group, then runs every config of `runs` (keyword arguments of _partitioned) on it;
+    rank 0 pickles the list of their gathered outputs to out_path (a file, not a queue: the parent reads it only after
+    joining the ranks, and a pipe would block a writer of more than its buffer until then)."""
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
-    dtype = getattr(torch, dtype_name)
     if backend == "nccl":
         torch.cuda.set_device(rank)
         dev = torch.device("cuda", rank)
         dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
-        ops = None
     else:
         dev = torch.device("cpu")
         dist.init_process_group("gloo", rank=rank, world_size=world)
-        ops = OracleOps()
     try:
-        mats, x, h, b = _case(G=G, F=F, K=K)
-        B, G, N = x.shape
-        F = h.shape[0]
-        gso = gnn_b200.SparseGSO.from_scipy(mats, dtype=dtype)
-        part = PartitionedLSIGF(gso, mode=mode, device=dev, ops=ops, grid=grid)
-        R = part.rows_per_rank
-        xn = torch.tensor(x, dtype=dtype).reshape(B * G, N).t().contiguous()       # node-major [N, B*G]
-        ht = torch.tensor(h, dtype=dtype, device=dev)
-        bt = torch.tensor(b, dtype=dtype, device=dev)
-        if mode == "grid":
-            x_local = part.grid_tile(xn, B, G).to(dev)
-        elif mode == "nodes":
-            xp = torch.zeros(part.n_pad, B * G, dtype=dtype)
-            xp[:N] = xn
-            x_local = xp[part.r0:part.r1].to(dev)
-        else:
-            g0, g1 = part.feature_slice(G)
-            x_local = xn.view(N, B, G)[:, :, g0:g1].reshape(N, B * (g1 - g0)).contiguous().to(dev)
-        if backend == "nccl":
-            # default construction under NCCL = the kernels move their rows over NVLink themselves; a silent fall back to
-            # the NCCL-collective path would leave the fused kernels untested
-            assert part.fused, "default PartitionedLSIGF under NCCL must take the fused path"
-        for _ in range(2):  # twice: buffers are reused across calls
-            y_local = part.forward(ht, x_local, bt, B=B)
-        assert tuple(y_local.shape) == (R, B * F)
-        if backend == "nccl" and G % (4 * world) == 0:
-            # the same step replayed as CUDA graphs (peer-flag fence, no NCCL inside): must reproduce the eager result
-            run = part.graphed(ht, x_local, bt, B=B)
-            for _ in range(3):
-                y_graph = run()
-            torch.cuda.synchronize()
-            assert torch.equal(y_graph, y_local), "graph replay differs from the eager fused step"
-        dx_nm = None
-        if backward:
-            # backward through the autograd wrapper (collective on every rank): dh, db summed over ranks, dx sharded like x
-            dy = np.random.default_rng(99).standard_normal((B, F, N))
-            dyp = torch.zeros(part.n_pad, B * F, dtype=dtype)
-            dyp[:N] = torch.tensor(dy, dtype=dtype).reshape(B * F, N).t()
-            hg, xg, bg = (t.clone().requires_grad_(True) for t in (ht, x_local, bt))
-            part.apply(hg, xg, bg, B).backward(dyp[part.r0:part.r1].to(dev))
-            if mode == "grid":
-                tiles = [torch.empty_like(xg.grad) for _ in range(world)]      # [rows_per_group, B*(G/P_c)] of rank (rg, cg)
-                dist.all_gather(tiles, xg.grad.contiguous())
-                Rr, Gl = part.rows_per_group, G // part.Pc
-                dx_full = torch.zeros(part.n_pad, B, G, dtype=dtype, device=dev)
-                for p_, t_ in enumerate(tiles):
-                    r_, c_ = p_ // part.Pc, p_ % part.Pc
-                    dx_full[r_ * Rr:(r_ + 1) * Rr, :, c_ * Gl:(c_ + 1) * Gl] = t_.reshape(Rr, B, Gl)
-                dx_nm = dx_full[:N]
-            elif mode == "nodes":
-                dxs = [torch.empty_like(xg.grad) for _ in range(world)]
-                dist.all_gather(dxs, xg.grad.contiguous())
-                dx_nm = torch.cat(dxs)[:N].reshape(N, B, G)
-            else:
-                per = (G + world - 1) // world
-                mine = torch.zeros(N, B, per, dtype=dtype, device=dev)
-                mine[:, :, :g1 - g0] = xg.grad.reshape(N, B, g1 - g0)
-                dxs = [torch.empty_like(mine) for _ in range(world)]
-                dist.all_gather(dxs, mine)
-                dx_nm = torch.cat(dxs, dim=2)[:, :, :G] if G % world == 0 else \
-                    torch.cat([d[:, :, :max(0, min(G, (p + 1) * per) - min(G, p * per))] for p, d in enumerate(dxs)], dim=2)
-        ys = [torch.empty_like(y_local) for _ in range(world)]
-        dist.all_gather(ys, y_local.contiguous())
+        outs = [_partitioned(rank, world, backend, dev, **cfg) for cfg in runs]
         if rank == 0:
-            y = torch.cat(ys)[:N].cpu().double().numpy().reshape(N, B, F).transpose(1, 2, 0)
-            npd = np.float32 if dtype == torch.float32 else np.float64
-            import scipy.sparse as sp
-            mr = [sp.csr_matrix((m.data.astype(npd).astype(np.float64), m.indices, m.indptr), shape=m.shape) for m in mats]
-            r64 = lambda a: a.astype(npd).astype(np.float64)  # noqa: E731
-            y_ref = orc.lsigf_sparse(r64(h), mr, r64(x), r64(b))
-            rel = lambda a, r: float(np.abs(a - r).max() / np.abs(r).max())  # noqa: E731
-            errs = [rel(y, y_ref)]
-            if backward:
-                dh_ref, dx_ref, db_ref = orc.lsigf_grads_sparse(r64(h), mr, r64(x), r64(dy), (F, 1))
-                errs += [rel(hg.grad.cpu().double().numpy(), dh_ref),
-                         rel(dx_nm.cpu().double().numpy().transpose(1, 2, 0), dx_ref),
-                         rel(bg.grad.cpu().double().numpy(), db_ref)]
-            result_q.put(max(errs))
+            with open(out_path, "wb") as f:
+                pickle.dump(outs, f)
     finally:
         dist.destroy_process_group()
 
 
-def _run(backend, mode, dtype_name, world=2, G=6, backward=True, F=8, grid=None, K=4):
-    ctx = mp.get_context("spawn")
+def _partitioned(rank, world, backend, dev, mode, dtype_name, G=6, backward=True, F=8, grid=None, K=4, trace=False):
+    """PartitionedLSIGF forward (twice: buffers are reused), its CUDA-graph replay where the fused path allows one, and
+    backward through part.apply; returns (rank 0) the outputs gathered over the ranks as fp64 arrays in the oracle's
+    layouts: y [B, F, N], and with backward dh [F, E, K, G], dx [B, G, N], db [F, 1].  trace: the hop kernels the first
+    forward and the backward launched are returned too, with whether the fused path ran and its arenas' kinds."""
+    import gnn_b200
+    from gnn_b200.distributed import PartitionedLSIGF
+    dtype = getattr(torch, dtype_name)
+    ops = OracleOps() if backend != "nccl" else None
+    mats, x, h, b = _case(G=G, F=F, K=K)
+    B, G, N = x.shape
+    F = h.shape[0]
+    gso = gnn_b200.SparseGSO.from_scipy(mats, dtype=dtype)
+    part = PartitionedLSIGF(gso, mode=mode, device=dev, ops=ops, grid=grid)
+    R = part.rows_per_rank
+    xn = torch.tensor(x, dtype=dtype).reshape(B * G, N).t().contiguous()       # node-major [N, B*G]
+    ht = torch.tensor(h, dtype=dtype, device=dev)
+    bt = torch.tensor(b, dtype=dtype, device=dev)
+    if mode == "grid":
+        x_local = part.grid_tile(xn, B, G).to(dev)
+    elif mode == "nodes":
+        xp = torch.zeros(part.n_pad, B * G, dtype=dtype)
+        xp[:N] = xn
+        x_local = xp[part.r0:part.r1].to(dev)
+    else:
+        g0, g1 = part.feature_slice(G)
+        x_local = xn.view(N, B, G)[:, :, g0:g1].reshape(N, B * (g1 - g0)).contiguous().to(dev)
+    if backend == "nccl":
+        # default construction under NCCL = the kernels move their rows over NVLink themselves; a silent fall back to
+        # the NCCL-collective path would leave the fused kernels untested
+        assert part.fused, "default PartitionedLSIGF under NCCL must take the fused path"
+    kernels = []
+
+    def traced(fn):
+        if not trace:
+            return fn()
+        from torch.profiler import ProfilerActivity, profile
+        from dispatch_harness import _norm
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            out = fn()
+            torch.cuda.synchronize()
+        kernels.extend(_norm(e.name).split("(")[0] for e in prof.events()
+                       if e.device_type == torch.autograd.DeviceType.CUDA and "b200gf::" in e.name)
+        return out
+
+    y_local = traced(lambda: part.forward(ht, x_local, bt, B=B))
+    y_local = part.forward(ht, x_local, bt, B=B)
+    assert tuple(y_local.shape) == (R, B * F)
+    if backend == "nccl" and G % (4 * world) == 0:
+        # the same step replayed as CUDA graphs (peer-flag fence, no NCCL inside): must reproduce the eager result
+        run = part.graphed(ht, x_local, bt, B=B)
+        for _ in range(3):
+            y_graph = run()
+        torch.cuda.synchronize()
+        assert torch.equal(y_graph, y_local), "graph replay differs from the eager fused step"
+    out = {}
+    if backward:
+        # backward through the autograd wrapper (collective on every rank): dh, db summed over ranks, dx sharded like x
+        dy = np.random.default_rng(99).standard_normal((B, F, N))
+        dyp = torch.zeros(part.n_pad, B * F, dtype=dtype)
+        dyp[:N] = torch.tensor(dy, dtype=dtype).reshape(B * F, N).t()
+        hg, xg, bg = (t.clone().requires_grad_(True) for t in (ht, x_local, bt))
+        traced(lambda: part.apply(hg, xg, bg, B).backward(dyp[part.r0:part.r1].to(dev)))
+        if mode == "grid":
+            tiles = [torch.empty_like(xg.grad) for _ in range(world)]      # [rows_per_group, B*(G/P_c)] of rank (rg, cg)
+            dist.all_gather(tiles, xg.grad.contiguous())
+            Rr, Gl = part.rows_per_group, G // part.Pc
+            dx_full = torch.zeros(part.n_pad, B, G, dtype=dtype, device=dev)
+            for p_, t_ in enumerate(tiles):
+                r_, c_ = p_ // part.Pc, p_ % part.Pc
+                dx_full[r_ * Rr:(r_ + 1) * Rr, :, c_ * Gl:(c_ + 1) * Gl] = t_.reshape(Rr, B, Gl)
+            dx_nm = dx_full[:N]
+        elif mode == "nodes":
+            dxs = [torch.empty_like(xg.grad) for _ in range(world)]
+            dist.all_gather(dxs, xg.grad.contiguous())
+            dx_nm = torch.cat(dxs)[:N].reshape(N, B, G)
+        else:
+            per = (G + world - 1) // world
+            mine = torch.zeros(N, B, per, dtype=dtype, device=dev)
+            mine[:, :, :g1 - g0] = xg.grad.reshape(N, B, g1 - g0)
+            dxs = [torch.empty_like(mine) for _ in range(world)]
+            dist.all_gather(dxs, mine)
+            dx_nm = torch.cat(dxs, dim=2)[:, :, :G] if G % world == 0 else \
+                torch.cat([d[:, :, :max(0, min(G, (p + 1) * per) - min(G, p * per))] for p, d in enumerate(dxs)], dim=2)
+        out.update(dh=hg.grad.cpu().double().numpy(), dx=dx_nm.cpu().double().numpy().transpose(1, 2, 0),
+                   db=bg.grad.cpu().double().numpy())
+    ys = [torch.empty_like(y_local) for _ in range(world)]
+    dist.all_gather(ys, y_local.contiguous())
+    out["y"] = torch.cat(ys)[:N].cpu().double().numpy().reshape(N, B, F).transpose(1, 2, 0)
+    if trace:
+        arenas = sorted({a.kind for a in part._arenas.values()} | ({"cuda-ipc"} if part._symm_by_width else set()))
+        out.update(kernels=sorted(set(kernels)), fused=part.fused, arenas=arenas)
+    return out if rank == 0 else None
+
+
+def _spawn(backend, world, runs):
     for attempt in range(3):                     # the rendezvous port is picked by bind-and-release: retry if someone took it
-        q = ctx.SimpleQueue()
-        try:
-            mp.spawn(_worker, args=(world, _free_port(), backend, mode, dtype_name, q, G, backward, F, grid, K), nprocs=world,
-                     join=True)
-            return q.get()
-        except Exception as exc:
-            if "EADDRINUSE" not in str(exc) or attempt == 2:
-                raise
+        with tempfile.TemporaryDirectory() as d:
+            path = os.path.join(d, "outs.pkl")
+            try:
+                mp.spawn(_worker, args=(world, _free_port(), backend, runs, path), nprocs=world, join=True)
+            except Exception as exc:
+                if "EADDRINUSE" not in str(exc) or attempt == 2:
+                    raise
+                continue
+            with open(path, "rb") as f:
+                return pickle.load(f)
+
+
+def _hold(out, dtype_name, G=6, backward=True, F=8, K=4):
+    """Holds a run's gathered outputs to orc.lsigf_envelope componentwise (fp32: with the 3xTF32 tensor-core
+    contraction's term) and returns their largest max-normalised error against the sparse fp64 oracle."""
+    import scipy.sparse as sp
+    mats, x, h, b = _case(G=G, F=F, K=K)
+    B, _, N = x.shape
+    npd = np.float32 if dtype_name == "float32" else np.float64
+    r64 = lambda a: a.astype(npd).astype(np.float64)  # noqa: E731
+    mr = [sp.csr_matrix((r64(m.data), m.indices, m.indptr), shape=m.shape) for m in mats]
+    dy = r64(np.random.default_rng(99).standard_normal((B, h.shape[0], N)))
+    env = orc.lsigf_envelope(r64(h), mr, r64(x), r64(b), dy, npd, tf32x3=npd == np.float32)
+    refs = {"y": orc.lsigf_sparse(r64(h), mr, r64(x), r64(b))}
+    if backward:
+        refs.update(zip(("dh", "dx", "db"), orc.lsigf_grads_sparse(r64(h), mr, r64(x), dy, (h.shape[0], 1))))
+    errs = []
+    for name, ref in refs.items():
+        v = orc.bound_violation(out[name], ref, env[name])
+        print("%s: worst error / bound %.3g" % (name, v))
+        assert v <= 1.0, "%s: error %.3g x its componentwise bound" % (name, v)
+        errs.append(float(np.abs(out[name] - ref).max() / np.abs(ref).max()))
+    return max(errs)
+
+
+def _run(backend, mode, dtype_name, world=2, G=6, backward=True, F=8, grid=None, K=4):
+    out, = _spawn(backend, world, [dict(mode=mode, dtype_name=dtype_name, G=G, backward=backward, F=F, grid=grid, K=K)])
+    return _hold(out, dtype_name, G=G, backward=backward, F=F, K=K)
 
 
 @pytest.mark.parametrize("mode,G", [("nodes", 6), ("features", 6), ("features", 5)])
@@ -253,6 +304,28 @@ def test_partitioned_grid_nccl_world2(grid, dtype_name, tol):
         pytest.skip("needs 2 GPUs")
     err = _run("nccl", "grid", dtype_name, G=48, backward=False, grid=grid)
     assert err < tol, err
+
+
+@pytest.mark.gpu
+def test_partitioned_nccl_world1_fused_paths():
+    """NCCL with a single rank on one GPU takes the fused path of every sharding: the node sharding's all-gather
+    (bcast_rows for the k = 0 rows, EPI_BCAST hops, the locally stored last hop, the peer-flag fence, forward and backward
+    chains), the feature sharding's scatter (EPI_SCATTER) and the 2-D grid's (EPI_GRID), in fp32 and fp64, all in one
+    spawned process.  Each runs forward twice (reused arenas), its CUDA-graph replay and backward through part.apply;
+    the epilogue kernels must have launched, and y, dh, dx and db are held to the componentwise envelope.  One rank
+    hides cross-rank offsets (one peer, row0 = 0): tests/test_peer_epilogues.py covers those with simulated peers."""
+    runs = [dict(mode=m, dtype_name=d, G=48, F=24, K=4, backward=True, grid=(1, 1) if m == "grid" else None, trace=True)
+            for m in ("nodes", "features", "grid") for d in ("float32", "float64")]
+    want = {"nodes": [r"spmm_hop_v2_kernel<[\w,]*,2,1>", r"bcast_rows_kernel<"],
+            "features": [r"spmm_hop_v2_kernel<[\w,]*,1,1>"],
+            "grid": [r"spmm_hop_v2_kernel<[\w,]*,3,1>", r"bcast_rows_kernel<", r"scatter_rows_kernel<"]}
+    import re
+    for cfg, out in zip(runs, _spawn("nccl", 1, runs)):
+        print("%s %s: arenas %s, kernels %s" % (cfg["mode"], cfg["dtype_name"], out["arenas"], out["kernels"]))
+        assert out["fused"]
+        for k in want[cfg["mode"]]:
+            assert any(re.search(k, n) for n in out["kernels"]), "%s: %s did not launch" % (cfg["mode"], k)
+        _hold(out, cfg["dtype_name"], G=48, F=24, K=4)
 
 
 def test_unpack_tap_grads_is_the_adjoint_of_pack_taps():

@@ -717,10 +717,10 @@ CASES = (_hop_rows() + _contract_rows() + _tap_grad_rows() + _bias_grad_rows() +
 
 # __global__ functions of this table's sources without a case here, and where they are tested
 EXCLUDED = {
-    "peer_signal_kernel": "multi-process peer fence: tests/test_distributed.py",
-    "peer_wait_kernel": "multi-process peer fence: tests/test_distributed.py",
-    "bcast_rows_kernel": "all-gather epilogue of the node-sharded path: tests/test_cabi.py, tests/test_distributed.py",
-    "scatter_rows_kernel": "scatter epilogue of the feature-sharded path: tests/test_cabi.py, tests/test_distributed.py",
+    "peer_signal_kernel": "peer fence: tests/test_peer_epilogues.py (one participant), tests/test_distributed.py",
+    "peer_wait_kernel": "peer fence: tests/test_peer_epilogues.py (one participant), tests/test_distributed.py",
+    "bcast_rows_kernel": "all-gather of the node-sharded path's k = 0 rows: tests/test_peer_epilogues.py",
+    "scatter_rows_kernel": "scatter of the feature-sharded path's k = 0 slices: tests/test_peer_epilogues.py",
     "narrow_rowptr_kernel": "device plan build (b200gf_plan_create_device): tests/test_widen_*",
 }
 
