@@ -203,7 +203,8 @@ static int hop_chunk_lanes(int64_t n_src, int nw, int64_t l2_bytes, bool spread)
 
 // Windowed hop over rows of at least 128 bytes (CsrDev::win_*): one launch per (128-byte column chunk, source window),
 // chunk-major then window-major on the stream, so that the gathers of a launch read one window's rows of one chunk, an
-// L2-sized range.  Window 0 stores its sums, every later window adds its sums into dst (EPI_ACCUM).  Four 32-byte lanes
+// L2-sized range.  Window 0 stores its sums, every later window adds its sums into dst (EPI_ACCUM: fp32 with L2 vector
+// reductions, fp64 by read-add-write).  Four 32-byte lanes
 // own a row's chunk and a warp works on 32 / GS rows (spmm_hop_multirow_v2_kernel); a window holds few entries per row,
 // so that with GS = 4 a row needs no cross-lane fold.  Written columns: [0, padded(C)), as the plain hop.
 template <typename T, int MODE>
@@ -246,7 +247,10 @@ static int launch_windows(int sm_count, const CsrDev& A, int64_t n_rows, const T
 // H100): 250k-row windows ran the N = 1M, 64-column fp32 hop in 2.43 against 2.56 ms, 200k and 333k rows in 2.47 and
 // 2.44, 125k rows (16 MB) in 2.65.  Every window after the first re-reads and re-writes the destination and the window
 // offsets, so the gain shrinks as windows are added: W = 4 (N = 1M) gained 5 % per hop, W = 8 (N = 2M) 1.4 % (5.67
-// against 5.60 ms); more windows were not measured and are not taken.
+// against 5.60 ms); more windows were not measured and are not taken.  Re-measured once fp32 windows added in the L2
+// instead of reading dst back: R = 250k still ran er1m fastest (1.81 ms; 200k 1.88, 333k 1.96, 125k 2.38).  At N = 2M
+// 333k-row windows (W = 6) ran 5.19 against 5.49 ms, with read-add-write as well (5.27 against 5.51), but they lose at
+// N = 1M, so the rule stays.
 int64_t hop_window_rows(int64_t n_src, int64_t l2_bytes, bool spread) {
   if (!spread || l2_bytes <= 0 || n_src * 128 <= l2_bytes) return 0;
   const int64_t R = l2_bytes * 5 / 8 / 128;

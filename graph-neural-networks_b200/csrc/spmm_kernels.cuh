@@ -19,6 +19,12 @@
 #include <stdint.h>
 #include <type_traits>
 
+// EPI_ACCUM with fp32 32-byte lanes (the windowed hop's windows after the first): 1 adds into dst with L2 vector
+// reductions, 0 reads, adds and stores (tools/hop_window_bench.py --variants builds both)
+#ifndef B200GF_HOP_WIN_RED
+#define B200GF_HOP_WIN_RED 1
+#endif
+
 namespace b200gf {
 
 template <typename T, int VEC>
@@ -111,6 +117,15 @@ __device__ __forceinline__ Acc<T, H> load_stream_16(const T* p) {
     a.v[0] = t.x; a.v[1] = t.y;
   }
   return a;
+}
+
+// *p += a for one 16-byte fp32 half, as a reduction in the L2 (red.add.v4.f32) with L2 policy `pol`.  The sum is
+// p[i] + a[i], the operands of the read-add-write it replaces and so the same bits, except that the reduction flushes
+// subnormal operands and results to zero.  Two adds to one address in a launch would land in either order, so the bits
+// would vary from run to run: each caller's address belongs to its lane alone, and the stream orders the launches.
+__device__ __forceinline__ void red_add_16(float* p, const Acc<float, 4>& a, uint64_t pol) {
+  asm volatile("red.relaxed.gpu.global.add.L2::cache_hint.v4.f32 [%0], {%1,%2,%3,%4}, %5;"
+               :: "l"(p), "f"(a.v[0]), "f"(a.v[1]), "f"(a.v[2]), "f"(a.v[3]), "l"(pol) : "memory");
 }
 
 constexpr unsigned FULL = 0xffffffffu;
@@ -391,17 +406,27 @@ __device__ __forceinline__ void hop_epilogue(const ScatterParam<T, MODE>& sp, T*
     Acc<T, H> a0, a1;
 #pragma unroll
     for (int i = 0; i < H; ++i) { a0.v[i] = acc.v[i]; a1.v[i] = acc.v[H + i]; }
-    if constexpr (MODE == EPI_ACCUM) {
-      // dst is read and written once per window: streaming (evict-first) accesses keep the gathered window in the L2.
-      // Both halves are read before either is written, so that the two reads are in flight together.
-      Acc<T, H> d0 = load_stream_16<T, H>(p), d1;
-      if (hi_ok) d1 = load_stream_16<T, H>(p + HI); else d1.zero();
+    if constexpr (MODE == EPI_ACCUM && sizeof(T) == 4 && B200GF_HOP_WIN_RED) {
+      // fp32: the L2 adds each half into dst and returns nothing, so dst is not read back to the SM, whose warps keep
+      // hiding the gathers' latency.  The evict-first policy matches the streaming stores below.  (There is no vector
+      // fp64 reduction.)
+      uint64_t pol;
+      asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+      red_add_16(p, a0, pol);
+      if (hi_ok) red_add_16(p + HI, a1, pol);
+    } else {
+      if constexpr (MODE == EPI_ACCUM) {
+        // dst is read and written once per window: streaming (evict-first) accesses keep the gathered window in the L2.
+        // Both halves are read before either is written, so that the two reads are in flight together.
+        Acc<T, H> d0 = load_stream_16<T, H>(p), d1;
+        if (hi_ok) d1 = load_stream_16<T, H>(p + HI); else d1.zero();
 #pragma unroll
-      for (int i = 0; i < H; ++i) { a0.v[i] = d0.v[i] + a0.v[i]; a1.v[i] = d1.v[i] + a1.v[i]; }
+        for (int i = 0; i < H; ++i) { a0.v[i] = d0.v[i] + a0.v[i]; a1.v[i] = d1.v[i] + a1.v[i]; }
+      }
+      constexpr int SHs = MODE == EPI_ACCUM ? 1 : SH;
+      store_vec<T, H, SHs>(p, a0);
+      if (hi_ok) store_vec<T, H, SHs>(p + HI, a1);
     }
-    constexpr int SHs = MODE == EPI_ACCUM ? 1 : SH;
-    store_vec<T, H, SHs>(p, a0);
-    if (hi_ok) store_vec<T, H, SHs>(p + HI, a1);
   }
 }
 

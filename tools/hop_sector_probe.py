@@ -11,10 +11,17 @@ loaded (same sectors, half the load instructions, wrong sums), and with split ha
 form runs about as fast as the adjacent one, the sectors bound the gather and splitting the halves cannot help; if it
 runs close to twice as fast, each half-sector load costs its own L2 request.
 
-    python tools/hop_sector_probe.py --libs parent.so,new.so [--probe-so probe.so] [--rounds 5] [--reps 10] [--out r.json]
+Reduce (--reduce er1m,er2m, fp32, windows of the plan's default size): how much of the windowed hop the destination's
+read-add-write costs, and what adding in the L2 saves.  The library's windowed hop (variant 3 of hop_sector_probe.cu)
+built with B200GF_HOP_WIN_RED=0 (every window after the first reads dst, adds and stores) and with the default
+B200GF_HOP_WIN_RED=1 (it adds with red.add.v4.f32 and reads nothing back), against the store-only split-halves gather
+(variant 2, wrong sums), alternated; and whether the two accumulating builds give bitwise-equal outputs.
 
---probe-so defaults to compiling tools/hop_sector_probe.cu into a temporary directory.  Prints the card, power limit
-and clocks before and after.
+    python tools/hop_sector_probe.py --libs parent.so,new.so [--probe-so probe.so] [--rounds 5] [--reps 10] [--out r.json]
+    python tools/hop_sector_probe.py --reduce er1m,er2m [--rounds 5] [--reps 10] [--out r.json]
+
+--probe-so defaults to compiling tools/hop_sector_probe.cu into a temporary directory (--reduce always builds its two).
+Prints the card, power limit and clocks before and after.
 """
 import argparse
 import ctypes
@@ -34,11 +41,20 @@ import bench  # noqa: E402
 from hop_window_bench import card, check, load_lib, stats  # noqa: E402
 
 
-def build_probe(out):
+def build_probe(out, flags=()):
     nvcc = os.environ.get("NVCC") or "nvcc"
     subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-shared", "-Xcompiler",
-                           "-fPIC", os.path.join(ROOT, "tools", "hop_sector_probe.cu"), "-o", out])
+                           "-fPIC", *flags, os.path.join(ROOT, "tools", "hop_sector_probe.cu"), "-o", out])
     return out
+
+
+def load_probe(path):
+    probe = ctypes.CDLL(path)
+    probe.probe_window_hop.restype = ctypes.c_int
+    probe.probe_window_hop.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                       ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                       ctypes.c_int, ctypes.c_void_p]
+    return probe
 
 
 def timed(fn, reps):
@@ -120,11 +136,7 @@ def control(name, probe_path, rows, rounds, reps):
     dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
     rp_d, c_d, v_d = dev(rp), dev(wc), dev(wv)
     src = torch.randn(N, C, generator=torch.Generator().manual_seed(3)).cuda()
-    probe = ctypes.CDLL(probe_path)
-    probe.probe_window_hop.restype = ctypes.c_int
-    probe.probe_window_hop.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
-                                       ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
-                                       ctypes.c_int, ctypes.c_void_p]
+    probe = load_probe(probe_path)
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     st = torch.cuda.current_stream().cuda_stream
     names = {0: "adjacent halves", 1: "adjacent, first half only (control)", 2: "split halves (LaneMap)"}
@@ -147,15 +159,96 @@ def control(name, probe_path, rows, rounds, reps):
     return out
 
 
+def default_window_rows(name):
+    """Rows per window of the plan's default rule (hop_window_rows) for the workload's graph on this device."""
+    import torch
+    from gnn_b200.gso import Plan
+    w = bench.WORKLOADS[name]
+    plan = Plan.from_host_csr(bench.make_gso(w).csr, w["N"], torch.float32, torch.device("cuda", 0))
+    rows = int(plan.info(8))
+    del plan
+    return rows
+
+
+def reduce_probe(name, probes, rounds, reps):
+    """Store-only gather (variant 2) against the windowed hop (variant 3) of each build in `probes` ({label: path})."""
+    import torch
+    w = bench.WORKLOADS[name]
+    N, C = w["N"], w["B"] * w["G"]
+    rows = default_window_rows(name)
+    if rows == 0:
+        raise RuntimeError("%s builds no window copy on this device" % name)
+    r, c, v = bench.make_gso(w).csr[0]
+    rp, wc, wv, W = window_csr(np.asarray(r, np.int64), np.asarray(c, np.int32), np.asarray(v, np.float32), N, rows)
+    dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
+    rp_d, c_d, v_d = dev(rp), dev(wc), dev(wv)
+    src = torch.randn(N, C, generator=torch.Generator().manual_seed(3)).cuda()
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    st = torch.cuda.current_stream().cuda_stream
+    first = next(iter(probes))
+    arms = {"store only (control)": (load_probe(probes[first]), 2)}
+    arms.update({"windowed hop, %s" % k: (load_probe(p), 3) for k, p in probes.items()})
+    dst = {k: torch.empty(N, C, device="cuda") for k in arms}
+    ms = {k: [] for k in arms}
+
+    def hop(k):
+        probe, variant = arms[k]
+        if probe.probe_window_hop(variant, rp_d.data_ptr(), W, c_d.data_ptr(), v_d.data_ptr(), src.data_ptr(), C,
+                                  dst[k].data_ptr(), N, C, sms, st):
+            raise RuntimeError("probe_window_hop(%d) failed for %s" % (variant, k))
+
+    for _ in range(rounds):
+        for k in arms:
+            ms[k].append(timed(lambda: hop(k), reps))
+    hops = [k for k in arms if k.startswith("windowed")]
+    a, b = dst[hops[0]], dst[hops[-1]]
+    diff = (a.double() - b.double()).abs()
+    out = {"workload": bench.describe(w, "f32"), "window_rows": rows, "windows": W,
+           "destination_read_bytes": (W - 1) * N * C * 4, "arms": {k: stats(ms[k]) for k in arms},
+           "bitwise_equal": {"%s vs %s" % (hops[-1], hops[0]): bool(torch.equal(a, b))},
+           "max_abs_diff": float(diff.max()), "subnormal_outputs": int(((a != 0) & (a.abs() < 2.0 ** -126)).sum())}
+    print(json.dumps(out), flush=True)
+    del dst, src, rp_d, c_d, v_d
+    torch.cuda.empty_cache()
+    return out
+
+
+def main_reduce(args):
+    from gnn_b200 import _cabi
+    _cabi.load()
+    report = {"card": card(), "reduce": []}
+    print("card:", report["card"], flush=True)
+    with tempfile.TemporaryDirectory() as tmp:
+        probes = {"read-add-write (B200GF_HOP_WIN_RED=0)": build_probe(os.path.join(tmp, "red0.so"),
+                                                                       ["-DB200GF_HOP_WIN_RED=0"]),
+                  "L2 reduction (B200GF_HOP_WIN_RED=1)": build_probe(os.path.join(tmp, "red1.so"))}
+        for name in (s for s in args.reduce.split(",") if s):
+            report["reduce"].append(reduce_probe(name, probes, args.rounds, args.reps))
+    report["card_after"] = card()
+    print("card:", report["card_after"])
+    if args.out:
+        with open(args.out, "w") as f:
+            json.dump(report, f, indent=1)
+    for rs in report["reduce"]:
+        for k, a in rs["arms"].items():
+            print("%-40s %-45s %.3f ms [%.3f, %.3f]" % (rs["workload"][:40], k, a["median_ms"], a["min_ms"], a["max_ms"]))
+        print("  bitwise equal:", rs["bitwise_equal"], "max |diff|:", rs["max_abs_diff"])
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--libs", required=True, help="comma-separated libb200gf builds; the first is the baseline")
+    ap.add_argument("--libs", default="", help="comma-separated libb200gf builds; the first is the baseline")
+    ap.add_argument("--reduce", default="", help="comma-separated workloads of the destination reduce probe (no --libs)")
     ap.add_argument("--workload", default="er1m")
     ap.add_argument("--probe-so", default="", help="tools/hop_sector_probe.cu built as a shared library")
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--out", help="also write the report as JSON here")
     args = ap.parse_args()
+    if args.reduce:
+        return main_reduce(args)
+    if not args.libs:
+        ap.error("--libs or --reduce is required")
     import torch
     from gnn_b200 import _cabi
     _cabi.load()

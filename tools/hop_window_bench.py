@@ -9,7 +9,7 @@ spreads (min, max) in ms.
 
     python tools/hop_window_bench.py [--hops er1m] [--f64-hops er1m] [--rows 125000,200000,250000,333000]
                                      [--libs a.so,b.so] [--fwd er1m,er2m] [--f64 er1m] [--rounds 5] [--out r.json]
-    python tools/hop_window_bench.py --variants DIR   # builds the GS x U x HINT variant libraries into DIR and exits
+    python tools/hop_window_bench.py --variants DIR   # builds the variant libraries (GS x U x HINT, and RED=0) into DIR
 """
 import argparse
 import ctypes
@@ -34,11 +34,12 @@ def card():
         return "unknown (%s)" % exc
 
 
-VARIANTS = [(gs, u, hint) for gs in (4, 8) for u in (2, 4) for hint in (1, 3)]
+# (GS, U, HINT, RED): the geometry and L2 policy grid, and the library's geometry with read-add-write accumulation
+VARIANTS = [(gs, u, hint, 1) for gs in (4, 8) for u in (2, 4) for hint in (1, 3)] + [(4, 4, 3, 0)]
 
 
 def build_variants(outdir):
-    """Relinks the library once per windowed-hop geometry (B200GF_HOP_WIN_GS / _U / _HINT); only spmm.cu differs."""
+    """Relinks the library once per windowed-hop variant (B200GF_HOP_WIN_GS / _U / _HINT / _RED); only spmm.cu differs."""
     import importlib.util
     spec = importlib.util.spec_from_file_location("b200gf_build", os.path.join(ROOT, "graph-neural-networks_b200", "build.py"))
     b = importlib.util.module_from_spec(spec)
@@ -47,11 +48,12 @@ def build_variants(outdir):
     objdir = os.path.join(b.HERE, "build")
     others = [os.path.join(objdir, os.path.basename(s) + ".o") for s in b.SOURCES if s != "spmm.cu"]
     os.makedirs(outdir, exist_ok=True)
-    for gs, u, hint in VARIANTS:
-        tag = "gs%d_u%d_h%d" % (gs, u, hint)
+    for gs, u, hint, red in VARIANTS:
+        tag = "gs%d_u%d_h%d_red%d" % (gs, u, hint, red)
         o = os.path.join(outdir, "spmm_%s.o" % tag)
         subprocess.check_call([b._nvcc()] + b.NVCC_FLAGS + ["-DB200GF_HOP_WIN_GS=%d" % gs, "-DB200GF_HOP_WIN_U=%d" % u,
-                                                            "-DB200GF_HOP_WIN_HINT=%d" % hint, "-c",
+                                                            "-DB200GF_HOP_WIN_HINT=%d" % hint,
+                                                            "-DB200GF_HOP_WIN_RED=%d" % red, "-c",
                                                             os.path.join(b.CSRC, "spmm.cu"), "-o", o])
         subprocess.check_call([b._nvcc(), "-shared", "-o", os.path.join(outdir, "libb200gf_%s.so" % tag), o] + others +
                               ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"])
