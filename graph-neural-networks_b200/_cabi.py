@@ -5,10 +5,13 @@ There is NO fallback: if the library is missing `load()` raises, and every LSIGF
 import ctypes
 import os
 
+import torch
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libb200gf.so")
 
 F32, F64 = 0, 1
+DTYPE = {torch.float32: F32, torch.float64: F64}      # the dtypes the kernels run in, as the ABI's enum
 FEATURE_MAJOR, NODE_MAJOR = 0, 1
 HOP_FWD, HOP_BWD = 0, 1
 ACT_NONE, ACT_RELU = 0, 1
@@ -114,6 +117,11 @@ def load():
         fn.argtypes = args
     _lib = lib
     return lib
+
+
+def stream():
+    """The current CUDA stream's handle: every entry point enqueues its launches there."""
+    return torch.cuda.current_stream().cuda_stream
 
 
 def check(rc):

@@ -22,7 +22,7 @@ by building Sbar^-1 S~ as [F, E, P, G, N, N] dense tensors (205 GB each at F = G
     accumulated by arma.cu's element-wise kernels (b200gf_arma_forward / _backward).
 
 The choice is made per edge feature from the GSO (`ArmaOperator`), and both paths sum into one output.  The residue term
-and the bias are b200gf_forward / b200gf_backward on the plan of S.  CPU tensors raise; there is no dense fallback.
+and the bias are the LSIGF forward and backward on the plan of S.  CPU tensors raise; there is no dense fallback.
 """
 import math
 import weakref
@@ -33,7 +33,8 @@ import torch
 import torch.nn as nn
 
 from . import _cabi
-from .graphML import LSIGF, _ENUM, _as_bcn_view, _bias_2d, _stream, node_major_ld, padded_ld, to_node_major
+from .graphML import (LSIGF, _as_bcn_view, _bias_2d, _grad_in_input_layout, _lsigf_backward_nm, _lsigf_forward_nm,
+                      _workspace, check_operands, node_major_ld, plan_on, to_node_major)
 from .gso import Plan, SparseGSO, _dense_key, dense_to_csr, plan_for
 
 
@@ -142,8 +143,8 @@ def arma_operator(S):
 # ---------------------------------------------------------------------------------------------------------------
 class _ARMAFunction(torch.autograd.Function):
     """u = LSIGF(phi, S, x) + b + the ARMA chains of the edge features of `aplan` (psi, varphi: [F, E', P, G] for those
-    edge features, d: their diagonals [E', N]).  The H3 term and the bias are written by b200gf_forward, the chains are
-    added in place by b200gf_arma_forward; the backward mirrors it."""
+    edge features, d: their diagonals [E', N]).  The H3 term and the bias are written by the LSIGF forward, the chains
+    are added in place by b200gf_arma_forward; the backward mirrors it."""
 
     @staticmethod
     def forward(ctx, psi, varphi, phi, x, b, hplan, aplan, d, tMax, keep):
@@ -151,32 +152,20 @@ class _ARMAFunction(torch.autograd.Function):
         F_, _, P, G = psi.shape
         K = phi.shape[2]
         B, _, N = x.shape
-        dt = x.dtype
         psic, varc, phic = psi.contiguous(), varphi.contiguous(), phi.contiguous()
         ctx.x_node_major = node_major_ld(x) is not None
         xn, x_ld = to_node_major(x)
-        bias_per_node = 0
-        bc = None
-        if b is not None:
-            bias_per_node = 0 if b.shape[1] == 1 else 1
-            bc = b.contiguous()
-        ldf = padded_ld(B * F_, dt)
-        ybuf = torch.empty((N, ldf), dtype=dt, device=x.device)
-        ws_bytes = lib.b200gf_workspace_bytes(hplan.handle, B, G, F_, K, _cabi.NODE_MAJOR, 0)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=x.device)
-        _cabi.check(lib.b200gf_forward(hplan.handle, xn.data_ptr(), _cabi.NODE_MAJOR, x_ld, phic.data_ptr(),
-                                       None if bc is None else bc.data_ptr(), bias_per_node, ybuf.data_ptr(),
-                                       _cabi.NODE_MAJOR, ldf, ws.data_ptr(), ws_bytes, B, G, F_, K, _stream()))
+        ybuf, ldf, bias_per_node = _lsigf_forward_nm(hplan, phic, xn, x_ld, b, B, G, F_, K, _cabi.ACT_NONE)
         states = None
         if keep:
             st_bytes = lib.b200gf_arma_workspace_bytes(aplan.handle, B, G, F_, P, tMax, 3)
-            states = torch.empty((max(st_bytes, 1),), dtype=torch.uint8, device=x.device)
+            states = _workspace(max(st_bytes, 1), x.device)
         aws_bytes = lib.b200gf_arma_workspace_bytes(aplan.handle, B, G, F_, P, tMax, 1 if keep else 0)
-        aws = torch.empty((aws_bytes,), dtype=torch.uint8, device=x.device)
+        aws = _workspace(aws_bytes, x.device)
         _cabi.check(lib.b200gf_arma_forward(aplan.handle, d.data_ptr(), psic.data_ptr(), varc.data_ptr(), tMax, B, G,
                                             F_, P, xn.data_ptr(), x_ld, ybuf.data_ptr(), ldf,
                                             None if states is None else states.data_ptr(), aws.data_ptr(), aws_bytes,
-                                            _stream()))
+                                            _cabi.stream()))
         ctx.hplan, ctx.aplan, ctx.x_ld, ctx.tMax = hplan, aplan, x_ld, tMax
         ctx.bias_per_node = bias_per_node
         ctx.bias_shape = None if b is None else tuple(b.shape)
@@ -190,35 +179,18 @@ class _ARMAFunction(torch.autograd.Function):
         lib = _cabi.load()
         psic, varc, phic, xn, d, states = ctx.saved_tensors
         B, G, F_, K, P, N = ctx.dims
-        dt = psic.dtype
         dun, du_ld = to_node_major(du)
         need_dx, need_db = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
-        dphi = torch.empty_like(phic)
-        ldc = padded_ld(B * G, dt)
-        dxbuf = torch.empty((N, ldc), dtype=dt, device=du.device) if need_dx else None
-        db = torch.empty(ctx.bias_shape, dtype=dt, device=du.device) if (ctx.bias_shape and need_db) else None
-        ws_bytes = lib.b200gf_workspace_bytes(ctx.hplan.handle, B, G, F_, K, _cabi.NODE_MAJOR, 1)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=du.device)
-        _cabi.check(lib.b200gf_backward(ctx.hplan.handle, dun.data_ptr(), _cabi.NODE_MAJOR, du_ld, xn.data_ptr(),
-                                        _cabi.NODE_MAJOR, ctx.x_ld, phic.data_ptr(),
-                                        None if dxbuf is None else dxbuf.data_ptr(), _cabi.NODE_MAJOR, ldc,
-                                        dphi.data_ptr(), None if db is None else db.data_ptr(), ctx.bias_per_node,
-                                        ws.data_ptr(), ws_bytes, B, G, F_, K, _stream()))
+        dxbuf, ldc, dphi, db = _lsigf_backward_nm(ctx.hplan, dun, du_ld, xn, ctx.x_ld, phic, need_dx, need_db,
+                                                  ctx.bias_shape, ctx.bias_per_node, B, G, F_, K)
         dpsi, dvarphi = torch.empty_like(psic), torch.empty_like(varc)
         aws_bytes = lib.b200gf_arma_workspace_bytes(ctx.aplan.handle, B, G, F_, P, ctx.tMax, 2)
-        aws = torch.empty((aws_bytes,), dtype=torch.uint8, device=du.device)
+        aws = _workspace(aws_bytes, du.device)
         _cabi.check(lib.b200gf_arma_backward(ctx.aplan.handle, d.data_ptr(), psic.data_ptr(), varc.data_ptr(), ctx.tMax,
                                              B, G, F_, P, dun.data_ptr(), du_ld, states.data_ptr(),
                                              None if dxbuf is None else dxbuf.data_ptr(), ldc, dpsi.data_ptr(),
-                                             dvarphi.data_ptr(), aws.data_ptr(), aws_bytes, _stream()))
-        dx = None
-        if need_dx:
-            if ctx.x_node_major:
-                dx = _as_bcn_view(dxbuf, B, G, N)
-            else:
-                dx = torch.empty((B, G, N), dtype=dt, device=du.device)
-                _cabi.check(lib.b200gf_to_feature_major(_ENUM[dt], dxbuf.data_ptr(), ldc, dx.data_ptr(), N, B * G,
-                                                        _stream()))
+                                             dvarphi.data_ptr(), aws.data_ptr(), aws_bytes, _cabi.stream()))
+        dx = _grad_in_input_layout(dxbuf, ldc, B, G, N, ctx.x_node_major) if need_dx else None
         return dpsi, dvarphi, dphi, dx, db, None, None, None, None, None
 
 
@@ -246,16 +218,7 @@ def _dispatch_cuda(psi, varphi, phi, S, x, b, tMax, path=None):
     constant-diagonal or the general path, summed into one output.  path = None chooses from the GSO; "general" runs
     every edge feature on the general path and "constant" every one on the constant path (each must be constant).
     `_dispatch` is the hook the CPU tests replace with the oracle to exercise the host logic around it."""
-    if x.device.type != "cuda":
-        raise RuntimeError("b200gf: jARMA needs CUDA tensors (there is no CPU fallback); got x on %s" % x.device)
-    if x.dtype not in _ENUM:
-        raise RuntimeError("b200gf: jARMA supports float32 and float64, got %s" % x.dtype)
-    if any(t.dtype != x.dtype for t in (psi, varphi, phi)) or S.dtype != x.dtype or (b is not None and b.dtype != x.dtype):
-        raise RuntimeError("b200gf: jARMA expects psi, varphi, phi, S, x, b of one dtype, got psi=%s S=%s x=%s"
-                           % (psi.dtype, S.dtype, x.dtype))
-    if any(t.device != x.device for t in (psi, varphi, phi)) or (b is not None and b.device != x.device):
-        raise RuntimeError("b200gf: jARMA expects psi, varphi, phi, x, b on one device, got psi=%s x=%s"
-                           % (psi.device, x.device))
+    check_operands("jARMA", x, (psi, varphi, phi, b), S)
     op = arma_operator(S)
     E = op.E
     if path is None:
@@ -269,7 +232,7 @@ def _dispatch_cuda(psi, varphi, phi, S, x, b, tMax, path=None):
     else:
         raise ValueError("b200gf: path must be None, 'general' or 'constant', got %r" % (path,))
     ge = [e for e in range(E) if e not in ce]
-    hplan = plan_for(S, x.device)
+    hplan = plan_on(S, x.device)
     if ge:
         idx = op.index(ge, x.device)
         keep = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (psi, varphi, phi, x, b))

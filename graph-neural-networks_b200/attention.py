@@ -33,7 +33,8 @@ import torch.nn as nn
 
 from . import _cabi
 from . import edgegated as _eg
-from .edgegated import EdgeGatePattern, _require_cuda, _ENUM
+from .edgegated import EdgeGatePattern
+from .graphML import check_operands
 from .gso import SparseGSO, _dense_key
 
 
@@ -42,16 +43,15 @@ class _Attention(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, s_src, s_dst, pat):
-        _require_cuda(s_src, "the graph attention")
+        check_operands("the graph attention", s_src, ())
         lib = _cabi.load()
         s_src, s_dst = s_src.contiguous(), s_dst.contiguous()
         N, Bs = s_src.shape
         mixer = _unit_mixer(s_src.device, s_src.dtype)
         alpha = torch.empty((pat.nnz, Bs), dtype=s_src.dtype, device=s_src.device)
-        st = torch.cuda.current_stream().cuda_stream
-        _cabi.check(lib.b200gf_attention_forward(_ENUM[s_src.dtype], N, pat.nnz, Bs, pat.m_rowptr.data_ptr(),
+        _cabi.check(lib.b200gf_attention_forward(_cabi.DTYPE[s_src.dtype], N, pat.nnz, Bs, pat.m_rowptr.data_ptr(),
                                                  pat.m_col.data_ptr(), s_src.data_ptr(), s_dst.data_ptr(),
-                                                 mixer.data_ptr(), alpha.data_ptr(), st))
+                                                 mixer.data_ptr(), alpha.data_ptr(), _cabi.stream()))
         ctx.pat = pat
         ctx.save_for_backward(s_src, s_dst, alpha)
         return alpha
@@ -67,12 +67,11 @@ class _Attention(torch.autograd.Function):
         dsig1 = torch.empty_like(s_src)
         dsig2 = torch.empty_like(s_src)
         mixer = _unit_mixer(s_src.device, s_src.dtype)
-        st = torch.cuda.current_stream().cuda_stream
-        _cabi.check(lib.b200gf_attention_backward(_ENUM[s_src.dtype], N, pat.nnz, Bs, pat.m_rowptr.data_ptr(),
+        _cabi.check(lib.b200gf_attention_backward(_cabi.DTYPE[s_src.dtype], N, pat.nnz, Bs, pat.m_rowptr.data_ptr(),
                                                   pat.m_col.data_ptr(), pat.mT_rowptr.data_ptr(),
                                                   pat.mT_perm.data_ptr(), s_src.data_ptr(), s_dst.data_ptr(),
                                                   mixer.data_ptr(), alpha.data_ptr(), dalpha.data_ptr(),
-                                                  dlogit.data_ptr(), dsig1.data_ptr(), dsig2.data_ptr(), st))
+                                                  dlogit.data_ptr(), dsig1.data_ptr(), dsig2.data_ptr(), _cabi.stream()))
         return dsig1, dsig2, None
 
 

@@ -25,6 +25,7 @@ import weakref
 import torch
 import torch.nn as nn
 
+from . import _cabi
 from . import graphML as _gml
 from .gso import Plan
 
@@ -92,10 +93,7 @@ def _plan_for_batch(S):
 
 def _filter_on_space_time_graph(h, S, x_big, b_big):
     """LSIGF over the M-node operator of `S`; x_big [1, G, M] (node-major view), b_big None / [F, 1] / [F, M]."""
-    if x_big.device.type != "cuda":
-        raise RuntimeError("b200gf: LSIGF_DB needs CUDA tensors (there is no CPU fallback); got x on %s" % x_big.device)
-    if x_big.dtype not in (torch.float32, torch.float64):
-        raise RuntimeError("b200gf: LSIGF_DB supports float32 and float64, got %s" % x_big.dtype)
+    _gml.check_operands("LSIGF_DB", x_big, (h, b_big), S)
     if S.device != x_big.device:
         raise RuntimeError("b200gf: GSO on %s but x on %s" % (S.device, x_big.device))
     return _gml._LSIGFFunction.apply(h, x_big, b_big, _plan_for_batch(S))
@@ -124,8 +122,6 @@ def LSIGF_DB(h, S, x, b=None):
     assert x.shape[1] == T
     assert x.shape[2] == G
     assert x.shape[3] == N
-    if h.dtype != x.dtype or S.dtype != x.dtype or (b is not None and b.dtype != x.dtype):
-        raise RuntimeError("b200gf: LSIGF_DB expects h, S, x, b of one dtype, got h=%s S=%s x=%s" % (h.dtype, S.dtype, x.dtype))
     M = B * T * N
     # space-time node-major input [M, G] (node index (b, t, n)), handed to the filter as a [1, G, M] view of it
     x_big = x.permute(0, 1, 3, 2).reshape(M, G).t().unsqueeze(0)
@@ -236,25 +232,23 @@ class _HopFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, src, plan, o):
-        from . import _cabi
         if src.device.type != "cuda":
             raise RuntimeError("b200gf: GRNN_DB needs CUDA tensors (there is no CPU fallback); got the state on %s" % src.device)
         lib = _cabi.load()
         src = src.contiguous()
         dst = torch.empty_like(src)
         _cabi.check(lib.b200gf_hop(plan.handle, o, _cabi.HOP_FWD, src.data_ptr(), src.stride(0), dst.data_ptr(), dst.stride(0),
-                                   src.shape[1], _gml._stream()))
+                                   src.shape[1], _cabi.stream()))
         ctx.plan, ctx.o = plan, o
         return dst
 
     @staticmethod
     def backward(ctx, g):
-        from . import _cabi
         lib = _cabi.load()
         g = g.contiguous()
         out = torch.empty_like(g)
         _cabi.check(lib.b200gf_hop(ctx.plan.handle, ctx.o, _cabi.HOP_BWD, g.data_ptr(), g.stride(0), out.data_ptr(), out.stride(0),
-                                   g.shape[1], _gml._stream()))
+                                   g.shape[1], _cabi.stream()))
         return out, None, None
 
 

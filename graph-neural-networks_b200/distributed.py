@@ -31,14 +31,8 @@ import torch
 import torch.distributed as dist
 
 from . import _cabi
+from .graphML import padded_ld
 from .gso import Plan, SparseGSO
-
-_ENUM = {torch.float32: _cabi.F32, torch.float64: _cabi.F64}
-
-
-def _pad_ld(C, dtype):
-    q = 8 if dtype == torch.float32 else 4
-    return (C + q - 1) // q * q
 
 
 def row_slice(csr, r0, r1):
@@ -87,43 +81,40 @@ class CudaOps:
     def make_plan_full(self, gso):
         return gso.plan(self.device)
 
-    def _st(self):
-        return torch.cuda.current_stream().cuda_stream
-
     def hop(self, plan, e, direction, src, dst, C):
         _cabi.check(self.lib.b200gf_hop(plan.handle, e, direction, src.data_ptr(), src.stride(0), dst.data_ptr(),
-                                        dst.stride(0), C, self._st()))
+                                        dst.stride(0), C, _cabi.stream()))
 
     def hop_scatter(self, plan, e, direction, src, dst, C, peers, rows_per_peer, out_ld, out_col, gl, stride_b):
         _cabi.check(self.lib.b200gf_hop_scatter(plan.handle, e, direction, src.data_ptr(), src.stride(0), dst.data_ptr(),
                                                 dst.stride(0), C, _cabi.ptr_array(peers), len(peers), rows_per_peer,
-                                                out_ld, out_col, gl, stride_b, self._st()))
+                                                out_ld, out_col, gl, stride_b, _cabi.stream()))
 
     def scatter_rows(self, src, n_rows, C, peers, rows_per_peer, out_ld, out_col, gl, stride_b):
-        _cabi.check(self.lib.b200gf_scatter_rows(_ENUM[src.dtype], src.data_ptr(), src.stride(0), n_rows, C,
+        _cabi.check(self.lib.b200gf_scatter_rows(_cabi.DTYPE[src.dtype], src.data_ptr(), src.stride(0), n_rows, C,
                                                  _cabi.ptr_array(peers), len(peers), rows_per_peer, out_ld, out_col, gl,
-                                                 stride_b, self._st()))
+                                                 stride_b, _cabi.stream()))
 
     def hop_bcast(self, plan, e, direction, src, C, peers, mc, row0, out_ld):
         _cabi.check(self.lib.b200gf_hop_bcast(plan.handle, e, direction, src.data_ptr(), src.stride(0), C,
-                                              _cabi.ptr_array(peers), len(peers), mc or None, row0, out_ld, self._st()))
+                                              _cabi.ptr_array(peers), len(peers), mc or None, row0, out_ld, _cabi.stream()))
 
     def hop_grid(self, plan, e, direction, src, C, bc_peers, row0, bc_ld, sc_peers, rows_per_peer, out_ld, out_col, gl, stride_b):
         _cabi.check(self.lib.b200gf_hop_grid(plan.handle, e, direction, src.data_ptr(), src.stride(0), C,
                                              _cabi.ptr_array(bc_peers) if bc_peers else None, len(bc_peers), row0, bc_ld,
                                              _cabi.ptr_array(sc_peers), len(sc_peers), rows_per_peer, out_ld, out_col, gl,
-                                             stride_b, self._st()))
+                                             stride_b, _cabi.stream()))
 
     def bcast_rows(self, src, n_rows, C, peers, mc, row0, out_ld):
-        _cabi.check(self.lib.b200gf_bcast_rows(_ENUM[src.dtype], src.data_ptr(), src.stride(0), n_rows, C,
-                                               _cabi.ptr_array(peers), len(peers), mc or None, row0, out_ld, self._st()))
+        _cabi.check(self.lib.b200gf_bcast_rows(_cabi.DTYPE[src.dtype], src.data_ptr(), src.stride(0), n_rows, C,
+                                               _cabi.ptr_array(peers), len(peers), mc or None, row0, out_ld, _cabi.stream()))
 
     def pack_taps(self, h, transpose):
         F, E, K, G = h.shape
         T = 1 + E * (K - 1)
         W = torch.empty((T, F, G) if transpose else (T, G, F), dtype=h.dtype, device=h.device)
-        _cabi.check(self.lib.b200gf_pack_taps(_ENUM[h.dtype], h.contiguous().data_ptr(), W.data_ptr(), F, E, K, G,
-                                              1 if transpose else 0, self._st()))
+        _cabi.check(self.lib.b200gf_pack_taps(_cabi.DTYPE[h.dtype], h.contiguous().data_ptr(), W.data_ptr(), F, E, K, G,
+                                              1 if transpose else 0, _cabi.stream()))
         return W
 
     def tap_contract(self, zs, W, bias, out, n_rows, B, P, Q, bias_per_node=0):
@@ -131,19 +122,19 @@ class CudaOps:
         sb = self.lib.b200gf_tap_contract_scratch_bytes(T, P, Q)
         scratch = torch.empty(sb, dtype=torch.uint8, device=out.device)
         _cabi.check(self.lib.b200gf_tap_contract(
-            _ENUM[out.dtype], n_rows, B, P, Q, T, _cabi.ptr_array([z.data_ptr() for z in zs]),
+            _cabi.DTYPE[out.dtype], n_rows, B, P, Q, T, _cabi.ptr_array([z.data_ptr() for z in zs]),
             _cabi.i64_array([z.stride(0) for z in zs]), W.data_ptr(), None if bias is None else bias.data_ptr(),
-            bias_per_node, out.data_ptr(), out.stride(0), 0, scratch.data_ptr(), sb, self._st()))
+            bias_per_node, out.data_ptr(), out.stride(0), 0, scratch.data_ptr(), sb, _cabi.stream()))
 
     def tap_grad(self, A, vs, n_rows, B, P, Q):
         """dW[t][p][q] = sum_{n < n_rows, b} A[n, b*P + p] * vs[t][n, b*Q + q]   (b200gf_tap_grad)."""
         T = len(vs)
         dW = torch.empty((T, P, Q), dtype=A.dtype, device=A.device)
-        sb = self.lib.b200gf_tap_grad_scratch_bytes(_ENUM[A.dtype], n_rows, B, P, Q, T)
+        sb = self.lib.b200gf_tap_grad_scratch_bytes(_cabi.DTYPE[A.dtype], n_rows, B, P, Q, T)
         scratch = torch.empty(max(int(sb), 1), dtype=torch.uint8, device=A.device)
         _cabi.check(self.lib.b200gf_tap_grad(
-            _ENUM[A.dtype], n_rows, B, P, Q, T, A.data_ptr(), A.stride(0), _cabi.ptr_array([v.data_ptr() for v in vs]),
-            _cabi.i64_array([v.stride(0) for v in vs]), dW.data_ptr(), scratch.data_ptr(), sb, self._st()))
+            _cabi.DTYPE[A.dtype], n_rows, B, P, Q, T, A.data_ptr(), A.stride(0), _cabi.ptr_array([v.data_ptr() for v in vs]),
+            _cabi.i64_array([v.stride(0) for v in vs]), dW.data_ptr(), scratch.data_ptr(), sb, _cabi.stream()))
         return dW
 
 
@@ -426,7 +417,7 @@ class PartitionedLSIGF:
         C = x_rows.shape[1]
         B = C // G
         assert E == self.E and C == B * G and x_rows.shape[0] == self.rows_per_rank
-        ld = _pad_ld(C, self.dtype)
+        ld = padded_ld(C, self.dtype)
         R = self.rows_per_rank
         W = self.ops.pack_taps(h, False)
         # full-height sources for every hop that has a successor; the last hop of each e only needs local rows
@@ -448,7 +439,7 @@ class PartitionedLSIGF:
                     dist.all_gather_into_tensor(full.view(-1), dst_rows.reshape(-1), group=self.group)
                     src = full
                 zs.append(dst_rows)
-        y = torch.empty((R, _pad_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
+        y = torch.empty((R, padded_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
         bias = None
         if b is not None:
             assert b.shape[1] == 1, "per-node bias is not supported by the partitioned path"
@@ -459,7 +450,7 @@ class PartitionedLSIGF:
     # -- node sharding with the all-gather fused into the hop kernel ------------------------------------
     def _nodes_fused_ok(self, C):
         q = 8 if self.dtype == torch.float32 else 4
-        return C * (4 if self.dtype == torch.float32 else 8) > 128 and _pad_ld(C, self.dtype) % q == 0
+        return C * (4 if self.dtype == torch.float32 else 8) > 128 and padded_ld(C, self.dtype) % q == 0
 
     def _arena(self, key, n_bufs, ld):
         """Symmetric arena of n_bufs full-height node-major matrices [n_pad, ld] (cached per shape)."""
@@ -489,12 +480,12 @@ class PartitionedLSIGF:
         the last fence of this call: true for K >= 3 (fence after hop K-2 of the last chain), enforced for K == 2 by
         the trailing fence below."""
         C = rows.shape[1]
-        ld = _pad_ld(C, self.dtype)
+        ld = padded_ld(C, self.dtype)
         es = rows.element_size()
         T = 1 + E * (K - 1)
         R, r0 = self.rows_per_rank, self.r0
         ar = self._arena((key, ld, T), T, ld)
-        st = self.ops._st()
+        st = _cabi.stream()
         local_rows = lambda t: ar.local(t * ar.buf_bytes + r0 * ld * es, ld)      # noqa: E731
         local_full = lambda t: ar.local(t * ar.buf_bytes, ld)                     # noqa: E731
         if K > 1:
@@ -530,7 +521,7 @@ class PartitionedLSIGF:
             x_rows = x_rows.contiguous()
         zs = self._chain_nodes_fused(_cabi.HOP_FWD, x_rows, E, K, "fwd")
         W = self.ops.pack_taps(h, False)
-        y = torch.empty((R, _pad_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
+        y = torch.empty((R, padded_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
         bias = None
         if b is not None:
             assert b.shape[1] == 1, "per-node bias is not supported by the partitioned path"
@@ -550,7 +541,7 @@ class PartitionedLSIGF:
         dW = self.ops.tap_grad(x_rows, vs, R, B, G, F)                          # [T, G, F]
         dist.all_reduce(dW, group=self.group)
         dh = _unpack_tap_grads(dW.transpose(1, 2), E, K)
-        dx = torch.empty((R, _pad_ld(C, self.dtype)), dtype=self.dtype, device=self.device)
+        dx = torch.empty((R, padded_ld(C, self.dtype)), dtype=self.dtype, device=self.device)
         self.ops.tap_contract(vs, self.ops.pack_taps(h, True), None, dx, R, B, F, G)
         return dh, dx[:, :C], (self._bias_grad(dy_rows, B, F) if want_db else None)
 
@@ -581,7 +572,7 @@ class PartitionedLSIGF:
         Rc, Rr = self.rows_per_rank, self.rows_per_group
         assert x_tile.shape[0] == Rr and x_tile.shape[1] == Cl
         T = 1 + E * (K - 1)
-        ld = _pad_ld(Cl, self.dtype)
+        ld = padded_ld(Cl, self.dtype)
         es = x_tile.element_size()
         row_elems = B * T * G
         key = ("grid", ld, T, row_elems)
@@ -602,7 +593,7 @@ class PartitionedLSIGF:
         sc = [ar.peers[p] + ar.op_off + pbuf * ar.op_bytes for p in row_group]
         row0 = self.rg * Rr
         g0 = self.cg * Gl
-        st = self.ops._st()
+        st = _cabi.stream()
         if x_tile.stride(1) != 1 or (x_tile.stride(0) * es) % 32 or x_tile.data_ptr() % 32:
             xt = self._buffers(("gx", Cl), (Rr, ld))
             xt[:, :Cl].copy_(x_tile)
@@ -622,7 +613,7 @@ class PartitionedLSIGF:
                 ar.fence(st)
                 src = local_full(t)
         W = self.ops.pack_taps(h, False).reshape(1, T * G, F)
-        y = torch.empty((Rc, _pad_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
+        y = torch.empty((Rc, padded_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
         bias = None
         if b is not None:
             assert b.shape[1] == 1, "per-node bias is not supported by the partitioned path"
@@ -665,7 +656,7 @@ class PartitionedLSIGF:
         assert x_tile.shape[0] == Rr and x_tile.shape[1] == Cl
         T = 1 + E * (K - 1)
         rowg, colg = self._grid_groups()
-        ld = _pad_ld(Cl, self.dtype)
+        ld = padded_ld(Cl, self.dtype)
         g0 = self.rg * Rr
         full0 = self._buffers(("gz0", Cl), (self.n_pad, ld))
         full0[g0:g0 + Rr, :Cl].copy_(x_tile)
@@ -701,7 +692,7 @@ class PartitionedLSIGF:
         Rc = self.rows_per_rank
         zrow = self._grid_operand(E, K, G, x_tile, B)
         W = self.ops.pack_taps(h, False).reshape(1, T * G, F)
-        y = torch.empty((Rc, _pad_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
+        y = torch.empty((Rc, padded_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
         bias = None
         if b is not None:
             assert b.shape[1] == 1, "per-node bias is not supported by the partitioned path"
@@ -735,7 +726,7 @@ class PartitionedLSIGF:
         dh = _unpack_tap_grads(dW, E, K)
         # ---- dx
         Wall = self.ops.pack_taps(h, True).permute(1, 0, 2).reshape(1, F, T * G).contiguous()
-        U = torch.empty((Rc, _pad_ld(B * T * G, self.dtype)), dtype=self.dtype, device=self.device)
+        U = torch.empty((Rc, padded_ld(B * T * G, self.dtype)), dtype=self.dtype, device=self.device)
         self.ops.tap_contract([dy_rows], Wall, None, U, Rc, B, F, T * G)
         send = U[:, :B * T * G].reshape(Rc, B, T, Pc, Gl).permute(3, 2, 0, 1, 4).contiguous()        # [Pc, T, Rc, B, Gl]
         if rowg is not None:
@@ -750,7 +741,7 @@ class PartitionedLSIGF:
                 g0, g1 = self.rg * Rr, (self.rg + 1) * Rr
                 rows = [row_slice(self._grid_gso.csr[e], g0, g1) for e in range(E)]
                 self._grid_bwd_plan = self.ops.make_plan_ops(rows, None, Rr, self.n_pad, self.dtype)    # S_e w: gather with rows of S_e
-            ld = _pad_ld(Cl, self.dtype)
+            ld = padded_ld(Cl, self.dtype)
             g0 = self.rg * Rr
             for e in range(E):
                 w = Ut[1 + e * (K - 1) + (K - 2)]                                   # W_{e,K-1} = U_{e,K-1}
@@ -782,7 +773,7 @@ class PartitionedLSIGF:
         R = self.rows_per_rank
         T = 1 + E * (K - 1)
         assert x_cols.shape[0] == self.N and x_cols.shape[1] == Cl
-        ld = _pad_ld(Cl, self.dtype)
+        ld = padded_ld(Cl, self.dtype)
         z0 = self._buffers(("fz0", Cl), (self.n_pad, ld))
         z0[:self.N, :Cl].copy_(x_cols)
         recv = self._buffers(("frecv", T, Cl), (T, P, R, ld))   # recv[t, p]: my rows, column slice of rank p
@@ -801,7 +792,7 @@ class PartitionedLSIGF:
         # [T, P, R, B, Gl] -> row-local operand [R, B, T*G] (column t*G + p*Gl + gl == t*G + g)
         zrow = recv[:, :, :, :Cl].reshape(T, P, R, B, Gl).permute(2, 3, 0, 1, 4).reshape(R, B * T * G)
         W = self.ops.pack_taps(h, False).reshape(1, T * G, F)
-        y = torch.empty((R, _pad_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
+        y = torch.empty((R, padded_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
         bias = None
         if b is not None:
             assert b.shape[1] == 1, "per-node bias is not supported by the partitioned path"
@@ -832,7 +823,7 @@ class PartitionedLSIGF:
         sy.step += 1
         peers = sy.peer_ptrs(buf)
         g0 = self.rank * Gl
-        ld = _pad_ld(Cl, self.dtype)
+        ld = padded_ld(Cl, self.dtype)
         vecb = 16
         if x_cols.stride(1) == 1 and (x_cols.stride(0) * x_cols.element_size()) % vecb == 0 and x_cols.data_ptr() % vecb == 0:
             z0 = x_cols                                 # the caller's buffer is the k = 0 source: no staging copy
@@ -848,11 +839,11 @@ class PartitionedLSIGF:
                 self.ops.hop_scatter(self.plan, e, _cabi.HOP_FWD, src, dst, Cl, peers, R, row_elems, t * G + g0, Gl, T * G)
                 src = dst
         if self.fence == "flags":
-            sy.fence(self.rank, self.ops._st())             # every rank's scatters precede its flag store
+            sy.fence(self.rank, _cabi.stream())             # every rank's scatters precede its flag store
         else:
             dist.all_reduce(self._flag, group=self.group)   # every rank's scatters precede its contribution
         W = self.ops.pack_taps(h, False).reshape(1, T * G, F)
-        y = torch.empty((R, _pad_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
+        y = torch.empty((R, padded_ld(B * F, self.dtype)), dtype=self.dtype, device=self.device)
         bias = None
         if b is not None:
             assert b.shape[1] == 1, "per-node bias is not supported by the partitioned path"
@@ -892,7 +883,7 @@ class PartitionedLSIGF:
         B = C // G
         CF = B * F
         assert E == self.E and C == B * G and x_rows.shape[0] == R and dy_rows.shape[1] == CF
-        ldf = _pad_ld(CF, self.dtype)
+        ldf = padded_ld(CF, self.dtype)
         full0 = self._buffers(("v0", CF), (self.n_pad, ldf))
         full0[self.r0:self.r1, :CF].copy_(dy_rows)
         dist.all_gather_into_tensor(full0.view(-1), full0[self.r0:self.r1].reshape(-1), group=self.group)
@@ -913,7 +904,7 @@ class PartitionedLSIGF:
         dW = self.ops.tap_grad(x_rows, vs, R, B, G, F)  # [T, G, F]: x_rows^T V_t over my rows
         dist.all_reduce(dW, group=self.group)
         dh = _unpack_tap_grads(dW.transpose(1, 2), E, K)
-        dx = torch.empty((R, _pad_ld(C, self.dtype)), dtype=self.dtype, device=self.device)
+        dx = torch.empty((R, padded_ld(C, self.dtype)), dtype=self.dtype, device=self.device)
         self.ops.tap_contract(vs, self.ops.pack_taps(h, True), None, dx, R, B, F, G)   # sum_t V_t H_t^T, row-local
         return dh, dx[:, :C], (self._bias_grad(dy_rows, B, F) if want_db else None)
 
@@ -933,8 +924,8 @@ class PartitionedLSIGF:
         Cl = B * Gl
         CF = B * F
         assert dy_rows.shape[1] == CF
-        ldf = _pad_ld(CF, self.dtype)
-        ld = _pad_ld(max(Cl, 1), self.dtype)
+        ldf = padded_ld(CF, self.dtype)
+        ld = padded_ld(max(Cl, 1), self.dtype)
         dyf = self._buffers(("bdy", CF), (self.n_pad, ldf))
         dyf[self.r0:self.r1, :CF].copy_(dy_rows)
         dist.all_gather_into_tensor(dyf.view(-1), dyf[self.r0:self.r1].reshape(-1), group=self.group)
@@ -960,7 +951,7 @@ class PartitionedLSIGF:
         # ---- dx: U[n, b, t, g] = sum_f dY[n, b, f] h_t[f, g] for my rows, every g
         Wt = self.ops.pack_taps(h, True)                                         # [T, F, G]
         Wall = Wt.permute(1, 0, 2).reshape(1, F, T * G).contiguous()
-        U = torch.empty((R, _pad_ld(B * T * G, self.dtype)), dtype=self.dtype, device=self.device)
+        U = torch.empty((R, padded_ld(B * T * G, self.dtype)), dtype=self.dtype, device=self.device)
         self.ops.tap_contract([dyf[self.r0:self.r1]], Wall, None, U, R, B, F, T * G)
         Uv = U[:, :B * T * G].reshape(R, B, T, G)
         if P * per != G:
@@ -1034,11 +1025,11 @@ class PartitionedLSIGF:
         Gl = g1 - g0
         R = self.rows_per_rank
         Cl = B * Gl
-        ldf = _pad_ld(B * F, self.dtype)
+        ldf = padded_ld(B * F, self.dtype)
         part = self._buffers(("part", B, F), (self.n_pad, ldf))
         if Gl > 0:
             assert x_cols.shape[0] == self.N and x_cols.shape[1] == Cl
-            ld = _pad_ld(Cl, self.dtype)
+            ld = padded_ld(Cl, self.dtype)
             z0 = self._buffers(("fz0", Cl), (self.N, ld))
             z0[:, :Cl].copy_(x_cols)
             zs = [z0]

@@ -32,10 +32,10 @@ import torch.nn as nn
 
 from . import _cabi
 from . import recurrent as _rec
+from .graphML import check_operands
 from .gso import SparseGSO
 
 zeroTolerance = 1e-9   # graphML.py:72
-_ENUM = {torch.float32: _cabi.F32, torch.float64: _cabi.F64}
 
 
 def _rowptr(rows, N):
@@ -217,28 +217,20 @@ class EdgeGatePattern:
         return hit
 
 
-def _require_cuda(t, what):
-    if t.device.type != "cuda":
-        raise RuntimeError("b200gf: %s needs CUDA tensors (there is no CPU fallback); got %s" % (what, t.device))
-    if t.dtype not in _ENUM:
-        raise RuntimeError("b200gf: %s runs in float32 / float64, got %s" % (what, t.dtype))
-
-
 class _Attention(torch.autograd.Function):
     """alpha [nnz, Bs] = sparse learnAttentionGSO (graphML.py:640-737, P = E = F = 1) of s [N, Bs] (node-major)."""
 
     @staticmethod
     def forward(ctx, s, mixer, pat):
-        _require_cuda(s, "the edge-gate attention")
+        check_operands("the edge-gate attention", s, ())
         lib = _cabi.load()
         s = s.contiguous()
         mixer = mixer.reshape(2).to(s.dtype).contiguous()
         N, Bs = s.shape
         alpha = torch.empty((pat.nnz, Bs), dtype=s.dtype, device=s.device)
-        st = torch.cuda.current_stream().cuda_stream
-        _cabi.check(lib.b200gf_egate_attention_forward(_ENUM[s.dtype], N, pat.nnz, Bs, pat.m_rowptr.data_ptr(),
+        _cabi.check(lib.b200gf_egate_attention_forward(_cabi.DTYPE[s.dtype], N, pat.nnz, Bs, pat.m_rowptr.data_ptr(),
                                                        pat.m_col.data_ptr(), s.data_ptr(), mixer.data_ptr(),
-                                                       alpha.data_ptr(), st))
+                                                       alpha.data_ptr(), _cabi.stream()))
         ctx.pat = pat
         ctx.save_for_backward(s, mixer, alpha)
         return alpha
@@ -253,12 +245,11 @@ class _Attention(torch.autograd.Function):
         dlogit = torch.empty_like(alpha)
         dsig1 = torch.empty_like(s)
         dsig2 = torch.empty_like(s)
-        st = torch.cuda.current_stream().cuda_stream
-        _cabi.check(lib.b200gf_egate_attention_backward(_ENUM[s.dtype], N, pat.nnz, Bs, pat.m_rowptr.data_ptr(),
+        _cabi.check(lib.b200gf_egate_attention_backward(_cabi.DTYPE[s.dtype], N, pat.nnz, Bs, pat.m_rowptr.data_ptr(),
                                                         pat.m_col.data_ptr(), pat.mT_rowptr.data_ptr(),
                                                         pat.mT_perm.data_ptr(), s.data_ptr(), mixer.data_ptr(),
                                                         alpha.data_ptr(), dalpha.data_ptr(), dlogit.data_ptr(),
-                                                        dsig1.data_ptr(), dsig2.data_ptr(), st))
+                                                        dsig1.data_ptr(), dsig2.data_ptr(), _cabi.stream()))
         ds = mixer[0] * dsig1 + mixer[1] * dsig2
         dmixer = torch.stack(((s * dsig1).sum(), (s * dsig2).sum()))
         return ds, dmixer, None
@@ -282,18 +273,17 @@ class _GatedHop(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, u, gate, pat):
-        _require_cuda(u, "the edge-gated hop")
+        check_operands("the edge-gated hop", u, ())
         lib = _cabi.load()
         N, Bs, C = u.shape
         if u.stride(2) != 1 or u.stride(1) != C:
             u = u.contiguous()
         out = torch.empty((N, Bs, C), dtype=u.dtype, device=u.device)
         t_val, _, _ = pat.values(u.dtype)
-        st = torch.cuda.current_stream().cuda_stream
-        _cabi.check(lib.b200gf_gated_hop_forward(_ENUM[u.dtype], N, Bs, C, pat.t_rowptr.data_ptr(), pat.t_col.data_ptr(),
-                                                 t_val.data_ptr(), pat.t_pos.data_ptr(), _gate_ptr(gate, u, pat),
-                                                 gate.stride(0), gate.stride(1), u.data_ptr(), _row_ld(u),
-                                                 out.data_ptr(), Bs * C, st))
+        _cabi.check(lib.b200gf_gated_hop_forward(_cabi.DTYPE[u.dtype], N, Bs, C, pat.t_rowptr.data_ptr(),
+                                                 pat.t_col.data_ptr(), t_val.data_ptr(), pat.t_pos.data_ptr(),
+                                                 _gate_ptr(gate, u, pat), gate.stride(0), gate.stride(1), u.data_ptr(),
+                                                 _row_ld(u), out.data_ptr(), Bs * C, _cabi.stream()))
         ctx.pat = pat
         ctx.save_for_backward(u, gate)
         return out
@@ -310,13 +300,12 @@ class _GatedHop(torch.autograd.Function):
         if du is None and (dg is None or pat.nnz == 0):          # nothing to write (an empty mask has no gate)
             return None, None if dg is None else dg.t(), None
         _, s_val, m_sval = pat.values(u.dtype)
-        st = torch.cuda.current_stream().cuda_stream
         _cabi.check(lib.b200gf_gated_hop_backward(
-            _ENUM[u.dtype], N, Bs, C, pat.s_rowptr.data_ptr(), pat.s_col.data_ptr(), s_val.data_ptr(),
+            _cabi.DTYPE[u.dtype], N, Bs, C, pat.s_rowptr.data_ptr(), pat.s_col.data_ptr(), s_val.data_ptr(),
             pat.s_pos.data_ptr(), pat.m_rowptr.data_ptr(), pat.m_col.data_ptr(), m_sval.data_ptr(),
             _gate_ptr(gate, u, pat), gate.stride(0), gate.stride(1), u.data_ptr(), _row_ld(u), dout.data_ptr(), Bs * C,
             None if du is None else du.data_ptr(), Bs * C, None if dg is None or pat.nnz == 0 else dg.data_ptr(), 1, Bs,
-            st))
+            _cabi.stream()))
         return du, None if dg is None else dg.t(), None
 
 

@@ -16,10 +16,9 @@ import torch
 import torch.nn as nn
 
 from . import _cabi
-from .graphML import LSIGF
+from .graphML import LSIGF, check_operands
 
 zeroTolerance = 1e-9  # graphML.py:72
-_ENUM = {torch.float32: _cabi.F32, torch.float64: _cabi.F64}
 
 
 class EVStructure:
@@ -83,14 +82,14 @@ class _EVChain(torch.autograd.Function):
         B = xA.shape[0]
         w = w.contiguous()
         xT = xA.permute(1, 2, 0).contiguous()                                   # [G, NA, B]
-        st = torch.cuda.current_stream().cuda_stream
         train = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         n_states = max(K - 1, 1) if train else min(max(K - 1, 1), 2)
         states = torch.empty((n_states, F_ * G, NA, B), dtype=w.dtype, device=w.device)
         Y = torch.empty((F_, NA, B), dtype=w.dtype, device=w.device)
         diag = pe["diag"].data_ptr() if k0_identity else None
-        _cabi.check(lib.b200gf_ev_forward(_ENUM[w.dtype], NA, B, G, F_, K, pe["rowptr"].data_ptr(), pe["col"].data_ptr(), diag,
-                                          nnz, w.data_ptr(), xT.data_ptr(), states.data_ptr(), n_states, Y.data_ptr(), st))
+        _cabi.check(lib.b200gf_ev_forward(_cabi.DTYPE[w.dtype], NA, B, G, F_, K, pe["rowptr"].data_ptr(),
+                                          pe["col"].data_ptr(), diag, nnz, w.data_ptr(), xT.data_ptr(), states.data_ptr(),
+                                          n_states, Y.data_ptr(), _cabi.stream()))
         ctx.pe, ctx.NA, ctx.k0 = pe, NA, k0_identity
         ctx.save_for_backward(w, xT, states)
         return Y.permute(2, 0, 1)                                               # [B, F, NA] view
@@ -104,21 +103,20 @@ class _EVChain(torch.autograd.Function):
         B = xT.shape[2]
         assert states.shape[0] >= K - 1, "forward ran without gradients enabled"
         dY = dy.permute(1, 2, 0).contiguous()                                   # [F, NA, B]
-        st = torch.cuda.current_stream().cuda_stream
         lam = torch.empty((2, F_ * G, NA, B), dtype=w.dtype, device=w.device)
         dw = torch.zeros_like(w)
         dxT = torch.empty_like(xT)
         diag = pe["diag"].data_ptr() if ctx.k0 else None
-        _cabi.check(lib.b200gf_ev_backward(_ENUM[w.dtype], NA, B, G, F_, K, pe["rowptr"].data_ptr(), pe["col"].data_ptr(),
-                                           pe["rowptrT"].data_ptr(), pe["colT"].data_ptr(), pe["perm"].data_ptr(), diag, nnz,
-                                           w.data_ptr(), xT.data_ptr(), states.data_ptr(), dY.data_ptr(), lam.data_ptr(),
-                                           dw.data_ptr(), dxT.data_ptr(), st))
+        _cabi.check(lib.b200gf_ev_backward(_cabi.DTYPE[w.dtype], NA, B, G, F_, K, pe["rowptr"].data_ptr(),
+                                           pe["col"].data_ptr(), pe["rowptrT"].data_ptr(), pe["colT"].data_ptr(),
+                                           pe["perm"].data_ptr(), diag, nnz, w.data_ptr(), xT.data_ptr(),
+                                           states.data_ptr(), dY.data_ptr(), lam.data_ptr(), dw.data_ptr(),
+                                           dxT.data_ptr(), _cabi.stream()))
         return dw, dxT.permute(2, 0, 1), None, None, None
 
 
 def _require_cuda(x):
-    if x.device.type != "cuda":
-        raise RuntimeError("b200gf: EdgeVariantGF needs CUDA tensors (there is no CPU fallback); got x on %s" % x.device)
+    check_operands("EdgeVariantGF", x, ())
 
 
 def _run_chain(w, xA, pe, NA, k0_identity=False):
@@ -131,10 +129,7 @@ _chain = _run_chain      # the one hook the CPU tests replace (a dense torch cha
 def _evgf_sparse(Phi, struct, x, b, k0_identity=False):
     F_, E, K, G, N, _ = Phi.shape
     B = x.shape[0]
-    if x.device.type != "cuda":
-        raise RuntimeError("b200gf: EVGF needs CUDA tensors (there is no CPU fallback); got x on %s" % x.device)
-    if Phi.dtype != x.dtype or x.dtype not in _ENUM:
-        raise RuntimeError("b200gf: EVGF expects Phi and x of one dtype (float32 / float64)")
+    check_operands("EVGF", x, (Phi,))
     y = torch.zeros((B, F_, N), dtype=x.dtype, device=x.device)
     if struct.NA > 0:
         xA = x.index_select(2, struct.A)

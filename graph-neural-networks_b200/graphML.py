@@ -22,7 +22,6 @@ import torch.nn as nn
 from . import _cabi
 from .gso import Plan, SparseGSO, plan_for
 
-_ENUM = {torch.float32: _cabi.F32, torch.float64: _cabi.F64}
 _ELEMS_PER_SECTOR = {torch.float32: 8, torch.float64: 4}
 
 
@@ -50,10 +49,6 @@ def node_major_ld(t):
     return sn
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 def to_node_major(x):
     """[B, C, N] tensor -> (node-major buffer [N, ld], ld).  No copy when x already is such a view."""
     B, C, N = x.shape
@@ -64,7 +59,8 @@ def to_node_major(x):
     xc = x.contiguous()
     ld = padded_ld(B * C, x.dtype)
     buf = torch.empty((N, ld), dtype=x.dtype, device=x.device)
-    _cabi.check(lib.b200gf_to_node_major(_ENUM[x.dtype], xc.data_ptr(), buf.data_ptr(), ld, N, B * C, _stream()))
+    _cabi.check(lib.b200gf_to_node_major(_cabi.DTYPE[x.dtype], xc.data_ptr(), buf.data_ptr(), ld, N, B * C,
+                                         _cabi.stream()))
     return buf, ld
 
 
@@ -72,11 +68,12 @@ def to_feature_major(y):
     """[B, C, N] result (typically the permuted node-major view LSIGF returns) -> contiguous reference layout, with one
     coalesced tiled transpose (b200gf_to_feature_major) instead of an element-wise strided copy."""
     ld = node_major_ld(y)
-    if ld is None or y.device.type != "cuda" or y.dtype not in _ENUM:
+    if ld is None or y.device.type != "cuda" or y.dtype not in _cabi.DTYPE:
         return y.contiguous()
     B, C, N = y.shape
     out = torch.empty((B, C, N), dtype=y.dtype, device=y.device)
-    _cabi.check(_cabi.load().b200gf_to_feature_major(_ENUM[y.dtype], y.data_ptr(), ld, out.data_ptr(), N, B * C, _stream()))
+    _cabi.check(_cabi.load().b200gf_to_feature_major(_cabi.DTYPE[y.dtype], y.data_ptr(), ld, out.data_ptr(), N, B * C,
+                                                     _cabi.stream()))
     return out
 
 
@@ -85,38 +82,108 @@ def _as_bcn_view(buf, B, C, N):
     return buf[:, :B * C].view(N, B, C).permute(1, 2, 0)
 
 
+# ---------------------------------------------------------------------------------------------------
+# host code shared by the layer modules: operand checks and the node-major filter frame
+# ---------------------------------------------------------------------------------------------------
+def check_operands(name, x, tensors, S=None):
+    """Raises before any launch unless x is a CUDA tensor in a kernel dtype and every other operand the kernels read
+    (`tensors`, None entries skipped) has x's dtype and device; the GSO S (dense tensor, SparseGSO or Plan) needs only
+    x's dtype.  There is no CPU path, and a host tensor would reach a kernel as a host pointer."""
+    if x.device.type != "cuda":
+        raise RuntimeError("b200gf: %s needs CUDA tensors (there is no CPU fallback); got x on %s" % (name, x.device))
+    if x.dtype not in _cabi.DTYPE:
+        raise RuntimeError("b200gf: %s supports float32 and float64, got x in %s" % (name, x.dtype))
+    for t in (*tensors, S):
+        if t is not None and t.dtype != x.dtype:
+            # torch.matmul in the reference raises on mixed dtypes too ("expected scalar type ...")
+            raise RuntimeError("b200gf: %s expects its operands of one dtype, got %s and x in %s" % (name, t.dtype, x.dtype))
+    for t in tensors:
+        if t is not None and t.device != x.device:
+            raise RuntimeError("b200gf: %s expects its operands on one device, got %s and x on %s"
+                               % (name, t.device, x.device))
+
+
+def plan_on(S, device):
+    """plan_for(S, device), which must live on `device`."""
+    plan = plan_for(S, device)
+    if plan.device != device and not (plan.device.index == (device.index or 0)):
+        raise RuntimeError("b200gf: GSO plan lives on %s but x is on %s" % (plan.device, device))
+    return plan
+
+
+def _bias_arg(b):
+    """A [F, 1] or [F, N] bias as the entry points take it: (contiguous bias or None, bias_per_node)."""
+    if b is None:
+        return None, 0
+    return b.contiguous(), 0 if b.shape[1] == 1 else 1
+
+
+def _workspace(nbytes, device):
+    return torch.empty((nbytes,), dtype=torch.uint8, device=device)
+
+
+def _grad_in_input_layout(dxbuf, ldc, B, G, N, x_node_major):
+    """The input gradient [B, G, N] from its node-major buffer: a view of it when x was one (the producer of x reads it
+    through the same strides), else a contiguous tensor by one coalesced tiled transpose instead of a strided view
+    that autograd would re-copy element-wise."""
+    if x_node_major:
+        return _as_bcn_view(dxbuf, B, G, N)
+    dx = torch.empty((B, G, N), dtype=dxbuf.dtype, device=dxbuf.device)
+    _cabi.check(_cabi.load().b200gf_to_feature_major(_cabi.DTYPE[dx.dtype], dxbuf.data_ptr(), ldc, dx.data_ptr(), N,
+                                                     B * G, _cabi.stream()))
+    return dx
+
+
+def _lsigf_forward_nm(plan, hc, xn, x_ld, b, B, G, F_, K, act):
+    """One b200gf_forward_act on node-major x: returns the node-major output buffer [N, ldf], ldf and bias_per_node."""
+    lib = _cabi.load()
+    bc, bias_per_node = _bias_arg(b)
+    ldf = padded_ld(B * F_, xn.dtype)
+    ybuf = torch.empty((plan.n_rows, ldf), dtype=xn.dtype, device=xn.device)
+    ws_bytes = lib.b200gf_workspace_bytes(plan.handle, B, G, F_, K, _cabi.NODE_MAJOR, 0)
+    ws = _workspace(ws_bytes, xn.device)
+    _cabi.check(lib.b200gf_forward_act(plan.handle, xn.data_ptr(), _cabi.NODE_MAJOR, x_ld, hc.data_ptr(),
+                                       None if bc is None else bc.data_ptr(), bias_per_node,
+                                       ybuf.data_ptr(), _cabi.NODE_MAJOR, ldf, ws.data_ptr(), ws_bytes,
+                                       B, G, F_, K, int(act), _cabi.stream()))
+    return ybuf, ldf, bias_per_node
+
+
+def _lsigf_backward_nm(plan, dyn, dy_ld, xn, x_ld, hc, need_dx, need_db, bias_shape, bias_per_node, B, G, F_, K):
+    """One b200gf_backward on node-major dy and x: returns the node-major dx buffer (None unless need_dx), its ldc, the
+    tap gradient and the bias gradient (None without a bias or unless need_db)."""
+    lib = _cabi.load()
+    dt, dev = hc.dtype, dyn.device
+    dh = torch.empty_like(hc)
+    ldc = padded_ld(B * G, dt)
+    dxbuf = torch.empty((plan.n_rows, ldc), dtype=dt, device=dev) if need_dx else None
+    db = torch.empty(bias_shape, dtype=dt, device=dev) if (bias_shape is not None and need_db) else None
+    ws_bytes = lib.b200gf_workspace_bytes(plan.handle, B, G, F_, K, _cabi.NODE_MAJOR, 1)
+    ws = _workspace(ws_bytes, dev)
+    _cabi.check(lib.b200gf_backward(plan.handle, dyn.data_ptr(), _cabi.NODE_MAJOR, dy_ld,
+                                    xn.data_ptr(), _cabi.NODE_MAJOR, x_ld, hc.data_ptr(),
+                                    None if dxbuf is None else dxbuf.data_ptr(), _cabi.NODE_MAJOR, ldc,
+                                    dh.data_ptr(), None if db is None else db.data_ptr(), bias_per_node,
+                                    ws.data_ptr(), ws_bytes, B, G, F_, K, _cabi.stream()))
+    return dxbuf, ldc, dh, db
+
+
 class _LSIGFFunction(torch.autograd.Function):
     """y = LSIGF(h, S, x, b) with S fixed inside `plan` (graphML.py:83-176)."""
 
     @staticmethod
     def forward(ctx, h, x, b, plan, act=0):
-        lib = _cabi.load()
         F_, E, K, G = h.shape
         B, _, N = x.shape
-        dt = x.dtype
         hc = h.contiguous()
         ctx.x_node_major = node_major_ld(x) is not None
         xn, x_ld = to_node_major(x)
-        bias_per_node = 0
-        bc = None
-        if b is not None:
-            bias_per_node = 0 if b.shape[1] == 1 else 1
-            bc = b.contiguous()
-        ldf = padded_ld(B * F_, dt)
-        ybuf = torch.empty((N, ldf), dtype=dt, device=x.device)
-        ws_bytes = lib.b200gf_workspace_bytes(plan.handle, B, G, F_, K, _cabi.NODE_MAJOR, 0)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=x.device)
-        rc = lib.b200gf_forward_act(plan.handle, xn.data_ptr(), _cabi.NODE_MAJOR, x_ld, hc.data_ptr(),
-                                    None if bc is None else bc.data_ptr(), bias_per_node,
-                                    ybuf.data_ptr(), _cabi.NODE_MAJOR, ldf, ws.data_ptr(), ws_bytes,
-                                    B, G, F_, K, int(act), _stream())
-        _cabi.check(rc)
+        ybuf, ldf, bias_per_node = _lsigf_forward_nm(plan, hc, xn, x_ld, b, B, G, F_, K, act)
         ctx.act = int(act)
         ctx.ldf = ldf
         ctx.plan = plan
         ctx.x_ld = x_ld
         ctx.bias_per_node = bias_per_node
-        ctx.has_bias = b is not None
         ctx.bias_shape = None if b is None else tuple(b.shape)
         ctx.dims = (B, G, F_, K, E, N)
         if act:
@@ -127,45 +194,21 @@ class _LSIGFFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy):
-        lib = _cabi.load()
         if ctx.act:
             hc, xn, ybuf = ctx.saved_tensors
         else:
             hc, xn = ctx.saved_tensors
         B, G, F_, K, E, N = ctx.dims
-        plan = ctx.plan
-        dt = hc.dtype
         dyn, dy_ld = to_node_major(dy)
         if ctx.act:                                   # dy_pre = dy * (y > 0), one pass, node-major
-            masked = torch.empty((N, ctx.ldf), dtype=dt, device=dy.device)
-            _cabi.check(lib.b200gf_relu_backward(_ENUM[dt], ybuf.data_ptr(), ctx.ldf, dyn.data_ptr(), dy_ld,
-                                                 masked.data_ptr(), ctx.ldf, N, B * F_, _stream()))
+            masked = torch.empty((N, ctx.ldf), dtype=hc.dtype, device=dy.device)
+            _cabi.check(_cabi.load().b200gf_relu_backward(_cabi.DTYPE[hc.dtype], ybuf.data_ptr(), ctx.ldf, dyn.data_ptr(),
+                                                          dy_ld, masked.data_ptr(), ctx.ldf, N, B * F_, _cabi.stream()))
             dyn, dy_ld = masked, ctx.ldf
         need_dh, need_dx, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-        dh = torch.empty_like(hc)
-        ldc = padded_ld(B * G, dt)
-        dxbuf = torch.empty((N, ldc), dtype=dt, device=dy.device) if need_dx else None
-        db = None
-        if ctx.has_bias and need_db:
-            db = torch.empty(ctx.bias_shape, dtype=dt, device=dy.device)
-        ws_bytes = lib.b200gf_workspace_bytes(plan.handle, B, G, F_, K, _cabi.NODE_MAJOR, 1)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dy.device)
-        rc = lib.b200gf_backward(plan.handle, dyn.data_ptr(), _cabi.NODE_MAJOR, dy_ld,
-                                 xn.data_ptr(), _cabi.NODE_MAJOR, ctx.x_ld, hc.data_ptr(),
-                                 None if dxbuf is None else dxbuf.data_ptr(), _cabi.NODE_MAJOR, ldc,
-                                 dh.data_ptr(), None if db is None else db.data_ptr(), ctx.bias_per_node,
-                                 ws.data_ptr(), ws_bytes, B, G, F_, K, _stream())
-        _cabi.check(rc)
-        dx = None
-        if need_dx:
-            if ctx.x_node_major:
-                dx = _as_bcn_view(dxbuf, B, G, N)       # the producer of x reads it through the same strides
-            else:
-                # x was a plain [B, G, N] tensor: hand back a contiguous gradient (one coalesced tiled transpose)
-                # instead of a strided view that autograd would re-copy element-wise
-                dx = torch.empty((B, G, N), dtype=dt, device=dy.device)
-                _cabi.check(lib.b200gf_to_feature_major(_ENUM[dt], dxbuf.data_ptr(), ldc, dx.data_ptr(), N, B * G,
-                                                        _stream()))
+        dxbuf, ldc, dh, db = _lsigf_backward_nm(ctx.plan, dyn, dy_ld, xn, ctx.x_ld, hc, need_dx, need_db, ctx.bias_shape,
+                                                ctx.bias_per_node, B, G, F_, K)
+        dx = _grad_in_input_layout(dxbuf, ldc, B, G, N, ctx.x_node_major) if need_dx else None
         return (dh if need_dh else None), dx, db, None, None
 
 
@@ -216,21 +259,8 @@ def _bias_2d(b, F_, N, name):
 def _dispatch_cuda(h, S, x, b, act=0):
     """Device part of LSIGF: loud checks (there is no CPU path), plan lookup, the autograd function over the C ABI.
     `_dispatch` is the single hook the CPU tests replace with the oracle to exercise the argument handling above."""
-    if x.device.type != "cuda":
-        raise RuntimeError("b200gf: LSIGF needs CUDA tensors (there is no CPU fallback); got x on %s" % x.device)
-    if x.dtype not in _ENUM:
-        raise RuntimeError("b200gf: LSIGF supports float32 and float64, got %s" % x.dtype)
-    if h.dtype != x.dtype or S.dtype != x.dtype or (b is not None and b.dtype != x.dtype):
-        # torch.matmul in the reference raises on mixed dtypes too ("expected scalar type ...")
-        raise RuntimeError("b200gf: LSIGF expects h, S, x, b of one dtype, got h=%s S=%s x=%s" % (h.dtype, S.dtype, x.dtype))
-    if h.device != x.device or (b is not None and b.device != x.device):
-        # the kernels dereference h and b on the device: a host tensor here would hand them a host pointer
-        raise RuntimeError("b200gf: LSIGF expects h, x, b on one device, got h=%s x=%s b=%s"
-                           % (h.device, x.device, None if b is None else b.device))
-    plan = plan_for(S, x.device)
-    if plan.device != x.device and not (plan.device.index == (x.device.index or 0)):
-        raise RuntimeError("b200gf: GSO plan lives on %s but x is on %s" % (plan.device, x.device))
-    return _LSIGFFunction.apply(h, x, b, plan, act)
+    check_operands("LSIGF", x, (h, b), S)
+    return _LSIGFFunction.apply(h, x, b, plan_on(S, x.device), act)
 
 
 _dispatch = _dispatch_cuda

@@ -13,7 +13,6 @@ import torch
 
 from . import _cabi
 
-_TORCH2ENUM = {torch.float32: _cabi.F32, torch.float64: _cabi.F64}
 _NP2TORCH = {np.dtype("float32"): torch.float32, np.dtype("float64"): torch.float64}
 
 
@@ -159,7 +158,7 @@ class Plan:
         with torch.cuda.device(idx):
             torch.cuda.synchronize()
             rc = lib.b200gf_plan_create(ctypes.byref(out), idx, N, E, _cabi.ptr_array(rp), _cabi.ptr_array(ci),
-                                        _cabi.ptr_array(va), _TORCH2ENUM[dtype])
+                                        _cabi.ptr_array(va), _cabi.DTYPE[dtype])
         _cabi.check(rc)
         del keep
         return cls(out.value, N, N, E, dtype, torch.device("cuda", idx))
@@ -187,7 +186,7 @@ class Plan:
         out = ctypes.c_void_p()
         with torch.cuda.device(idx):
             rc = lib.b200gf_plan_create_ops(ctypes.byref(out), idx, n_rows, n_cols, len(fwd), f[0], f[1], f[2],
-                                            b[0], b[1], b[2], _TORCH2ENUM[dtype])
+                                            b[0], b[1], b[2], _cabi.DTYPE[dtype])
         _cabi.check(rc)
         return cls(out.value, n_rows, n_cols, len(fwd), dtype, torch.device("cuda", idx))
 
@@ -214,7 +213,7 @@ class Plan:
         with torch.cuda.device(idx):
             torch.cuda.current_stream().synchronize()          # the arrays were produced on the caller's stream
             rc = lib.b200gf_plan_create_device(ctypes.byref(out), idx, N, len(fwd), f[0], f[1], f[2], b[0], b[1], b[2],
-                                               _TORCH2ENUM[dtype])
+                                               _cabi.DTYPE[dtype])
         _cabi.check(rc)
         del keep
         return cls(out.value, N, N, len(fwd), dtype, torch.device("cuda", idx))

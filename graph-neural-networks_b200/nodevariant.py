@@ -25,7 +25,8 @@ import torch
 import torch.nn as nn
 
 from . import _cabi
-from .graphML import _ENUM, _as_bcn_view, _stream, node_major_ld, padded_ld, to_node_major
+from .graphML import (_as_bcn_view, _bias_arg, _grad_in_input_layout, _workspace, check_operands, node_major_ld,
+                      padded_ld, plan_on, to_node_major)
 from .gso import Plan, SparseGSO, plan_for
 
 zeroTolerance = 1e-9   # graphTools.py:45
@@ -156,26 +157,21 @@ class _NVGFFunction(torch.autograd.Function):
         F_, E, K, G, M = h.shape
         B, _, N = x.shape
         dt = x.dtype
-        enum = _ENUM[dt]
         hc = h.contiguous()
         ctx.x_node_major = node_major_ld(x) is not None
         xn, x_ld = to_node_major(x)
         node_tap, tap_rowptr, tap_nodes = taps.on(x.device)
         T = 1 + E * (K - 1)
         W = torch.empty((M, T, G, F_), dtype=dt, device=x.device)
-        _cabi.check(lib.b200gf_nv_pack_taps(enum, hc.data_ptr(), W.data_ptr(), F_, E, K, G, M, _stream()))
-        bias_per_node = 0
-        bc = None
-        if b is not None:
-            bias_per_node = 0 if b.shape[1] == 1 else 1
-            bc = b.contiguous()
+        _cabi.check(lib.b200gf_nv_pack_taps(_cabi.DTYPE[dt], hc.data_ptr(), W.data_ptr(), F_, E, K, G, M, _cabi.stream()))
+        bc, bias_per_node = _bias_arg(b)
         ldf = padded_ld(B * F_, dt)
         ybuf = torch.empty((N, ldf), dtype=dt, device=x.device)
         ws_bytes = lib.b200gf_nv_workspace_bytes(plan.handle, B, G, F_, K, M, 0)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=x.device)
+        ws = _workspace(ws_bytes, x.device)
         _cabi.check(lib.b200gf_nv_forward(plan.handle, xn.data_ptr(), x_ld, W.data_ptr(), node_tap.data_ptr(), M,
                                           None if bc is None else bc.data_ptr(), bias_per_node, ybuf.data_ptr(), ldf,
-                                          ws.data_ptr(), ws_bytes, B, G, F_, K, _stream()))
+                                          ws.data_ptr(), ws_bytes, B, G, F_, K, _cabi.stream()))
         ctx.plan, ctx.taps, ctx.x_ld = plan, taps, x_ld
         ctx.bias_per_node = bias_per_node
         ctx.bias_shape = None if b is None else tuple(b.shape)
@@ -197,20 +193,13 @@ class _NVGFFunction(torch.autograd.Function):
         dxbuf = torch.empty((N, ldc), dtype=dt, device=dy.device) if need_dx else None
         db = torch.empty(ctx.bias_shape, dtype=dt, device=dy.device) if (ctx.bias_shape and need_db) else None
         ws_bytes = lib.b200gf_nv_workspace_bytes(ctx.plan.handle, B, G, F_, K, M, 1)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dy.device)
+        ws = _workspace(ws_bytes, dy.device)
         _cabi.check(lib.b200gf_nv_backward(ctx.plan.handle, dyn.data_ptr(), dy_ld, xn.data_ptr(), ctx.x_ld, W.data_ptr(),
                                            node_tap.data_ptr(), M, tap_rowptr.data_ptr(), tap_nodes.data_ptr(),
                                            None if dxbuf is None else dxbuf.data_ptr(), ldc, dh.data_ptr(),
                                            None if db is None else db.data_ptr(), ctx.bias_per_node, ws.data_ptr(),
-                                           ws_bytes, B, G, F_, K, _stream()))
-        dx = None
-        if need_dx:
-            if ctx.x_node_major:
-                dx = _as_bcn_view(dxbuf, B, G, N)
-            else:
-                dx = torch.empty((B, G, N), dtype=dt, device=dy.device)
-                _cabi.check(lib.b200gf_to_feature_major(_ENUM[dt], dxbuf.data_ptr(), ldc, dx.data_ptr(), N, B * G,
-                                                        _stream()))
+                                           ws_bytes, B, G, F_, K, _cabi.stream()))
+        dx = _grad_in_input_layout(dxbuf, ldc, B, G, N, ctx.x_node_major) if need_dx else None
         return (dh if need_dh else None), dx, db, None, None
 
 
@@ -229,19 +218,8 @@ def _check_bias(b, F_, N):
 def _dispatch_cuda(h, S, x, b, taps):
     """Device part of NVGF: loud checks (there is no CPU path), plan lookup, the autograd function over the C ABI.
     `_dispatch` is the hook the CPU tests replace with the oracle to exercise the host logic around it."""
-    if x.device.type != "cuda":
-        raise RuntimeError("b200gf: NVGF needs CUDA tensors (there is no CPU fallback); got x on %s" % x.device)
-    if x.dtype not in _ENUM:
-        raise RuntimeError("b200gf: NVGF supports float32 and float64, got %s" % x.dtype)
-    if h.dtype != x.dtype or S.dtype != x.dtype or (b is not None and b.dtype != x.dtype):
-        raise RuntimeError("b200gf: NVGF expects h, S, x, b of one dtype, got h=%s S=%s x=%s" % (h.dtype, S.dtype, x.dtype))
-    if h.device != x.device or (b is not None and b.device != x.device):
-        raise RuntimeError("b200gf: NVGF expects h, x, b on one device, got h=%s x=%s b=%s"
-                           % (h.device, x.device, None if b is None else b.device))
-    plan = plan_for(S, x.device)
-    if plan.device != x.device and not (plan.device.index == (x.device.index or 0)):
-        raise RuntimeError("b200gf: GSO plan lives on %s but x is on %s" % (plan.device, x.device))
-    return _NVGFFunction.apply(h, x, b, plan, taps)
+    check_operands("NVGF", x, (h, b), S)
+    return _NVGFFunction.apply(h, x, b, plan_on(S, x.device), taps)
 
 
 _dispatch = _dispatch_cuda

@@ -31,10 +31,7 @@ class _MaxPoolFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, nb32, n_out, max_nb):
         from . import graphML as g
-        if x.device.type != "cuda":
-            raise RuntimeError("b200gf: MaxPoolLocal needs CUDA tensors (there is no CPU fallback); got x on %s" % x.device)
-        if x.dtype not in g._ENUM:
-            raise RuntimeError("b200gf: MaxPoolLocal supports float32 and float64, got %s" % x.dtype)
+        g.check_operands("MaxPoolLocal", x, ())
         lib = _cabi.load()
         B, F, Nin = x.shape
         ctx.x_node_major = g.node_major_ld(x) is not None
@@ -43,8 +40,8 @@ class _MaxPoolFunction(torch.autograd.Function):
         ld = g.padded_ld(C, x.dtype)
         out = torch.empty((n_out, ld), dtype=x.dtype, device=x.device)
         arg = torch.empty((n_out, C), dtype=torch.int32, device=x.device)
-        _cabi.check(lib.b200gf_maxpool_forward(g._ENUM[x.dtype], xn.data_ptr(), x_ld, Nin, C, nb32.data_ptr(), n_out, max_nb,
-                                               out.data_ptr(), ld, arg.data_ptr(), g._stream()))
+        _cabi.check(lib.b200gf_maxpool_forward(_cabi.DTYPE[x.dtype], xn.data_ptr(), x_ld, Nin, C, nb32.data_ptr(), n_out,
+                                               max_nb, out.data_ptr(), ld, arg.data_ptr(), _cabi.stream()))
         ctx.save_for_backward(arg)
         ctx.dims = (B, F, Nin, n_out, ld)
         return g._as_bcn_view(out, B, F, n_out)
@@ -58,8 +55,8 @@ class _MaxPoolFunction(torch.autograd.Function):
         dyn, dy_ld = g.to_node_major(dy)
         C = B * F
         dx = torch.empty((Nin, ld), dtype=dy.dtype, device=dy.device)
-        _cabi.check(lib.b200gf_maxpool_backward(g._ENUM[dy.dtype], dyn.data_ptr(), dy_ld, arg.data_ptr(), n_out, C,
-                                                dx.data_ptr(), ld, Nin, g._stream()))
+        _cabi.check(lib.b200gf_maxpool_backward(_cabi.DTYPE[dy.dtype], dyn.data_ptr(), dy_ld, arg.data_ptr(), n_out, C,
+                                                dx.data_ptr(), ld, Nin, _cabi.stream()))
         return g._as_bcn_view(dx, B, F, Nin), None, None, None
 
 
