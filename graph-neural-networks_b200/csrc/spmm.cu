@@ -12,6 +12,8 @@
 //   * operators with a window-major copy (million-node graphs): one launch per (128-byte column chunk, source window),
 //     each adding its window's sums into dst (launch_windows);
 //   * optional epilogue: the computed row slice is also stored over NVLink into a peer's buffer (b200gf_hop_scatter).
+// route_hop picks a hop's kernel, or refuses the hop, before any CUDA call; launch_route turns that choice into the
+// kernel's instantiation and launches it.
 #include <cstdlib>
 #include <cstring>
 
@@ -58,50 +60,67 @@ static BcastArgs<T> make_bcast(const BcastHost* bh) {
   return bc;
 }
 
-// Library configuration (tools/spmm_sweep.cu explores the alternatives): 256 threads, registers capped for 6 resident
-// blocks/SM (48 warps: the kernel is latency-bound below that), gathered rows loaded with an L2 evict_last policy and no
-// L1 allocation (a sticky subset of the gathered slab stays in L2), no next-row prefetch (it costs registers).
-template <typename T, int VEC, int L, int U>
-static int launch_one(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst,
-                      int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh) {
-  constexpr int THREADS = 256, MINB = sizeof(T) == 4 ? 6 : 4, HINT = 3;
-  constexpr bool PF = false;
-  auto kern = spmm_hop_kernel<T, VEC, L, U, THREADS, MINB, HINT, PF>;
-  const int n_chunks = (C + L * VEC - 1) / (L * VEC);
-  const int64_t n_items = n_rows * n_chunks;
-  if (n_items == 0) return B200GF_OK;
-  const int wpb = THREADS / 32;
+template <typename T, int EPI>
+static ScatterParam<T, EPI> make_epilogue(const ScatterHost* sh, const BcastHost* bh) {
+  ScatterParam<T, EPI> sp{};
+  if constexpr (EPI == EPI_SCATTER) sp.a = make_scatter<T>(sh);
+  if constexpr (EPI == EPI_BCAST) sp.a = make_bcast<T>(bh);
+  if constexpr (EPI == EPI_GRID) { sp.s = make_scatter<T>(sh); sp.a = make_bcast<T>(bh); }
+  return sp;
+}
+
+// one hop's operands; sh is null unless there are scatter peers, bh null without the all-gather epilogue
+template <typename T>
+struct HopArgs {
+  int sm_count;
+  const CsrDev& A;
+  int64_t n_rows;
+  const T* src;
+  int64_t src_ld;
+  T* dst;
+  int64_t dst_ld;
+  int C;
+  cudaStream_t st;
+  const ScatterHost* sh;
+  const BcastHost* bh;
+};
+
+// Launches kern as a persistent grid over `units` work items, `per_block` to a block: at most one resident wave
+// (sm_count x the kernel's occupancy), whose warps stride over the rest; chunks on blockIdx.y.
+template <typename T, typename K, typename... Args>
+static int launch_resident(K kern, int threads, const HopArgs<T>& h, int64_t units, int per_block, int chunks,
+                           Args... args) {
   int occ = 0;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, 0));
-  if (occ < 1) occ = 1;
-  int64_t blocks = (n_items + wpb - 1) / wpb;
-  const int64_t cap = (int64_t)sm_count * occ;  // one resident wave: persistent warps stride over the items
-  if (blocks > cap) blocks = cap;
-  kern<<<(unsigned)blocks, THREADS, 0, st>>>(A.rowptr, A.col, reinterpret_cast<const T*>(A.val), src, src_ld, dst,
-                                             dst_ld, n_rows, C, n_chunks, 1.0f, make_scatter<T>(sh));
+  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, 0));
+  const int64_t blocks = std::min<int64_t>((units + per_block - 1) / per_block, (int64_t)h.sm_count * std::max(occ, 1));
+  kern<<<dim3((unsigned)blocks, (unsigned)chunks), threads, 0, h.st>>>(args...);
   LAUNCH_CHECK();
   return B200GF_OK;
 }
 
+// Library configuration (tools/spmm_sweep.cu explores the alternatives): 256 threads, registers capped for 6 resident
+// blocks/SM (48 warps: the kernel is latency-bound below that), gathered rows loaded with an L2 evict_last policy and no
+// L1 allocation (a sticky subset of the gathered slab stays in L2), no next-row prefetch (it costs registers).
+template <typename T, int VEC, int L>
+static int launch_one(const HopArgs<T>& h) {
+  constexpr int U = 4, THREADS = 256, MINB = sizeof(T) == 4 ? 6 : 4, HINT = 3;
+  constexpr bool PF = false;
+  auto kern = spmm_hop_kernel<T, VEC, L, U, THREADS, MINB, HINT, PF>;
+  const int n_chunks = (h.C + L * VEC - 1) / (L * VEC);
+  return launch_resident(kern, THREADS, h, h.n_rows * n_chunks, THREADS / 32, 1, h.A.rowptr, h.A.col,
+                         reinterpret_cast<const T*>(h.A.val), h.src, h.src_ld, h.dst, h.dst_ld, h.n_rows, h.C, n_chunks,
+                         1.0f, make_scatter<T>(h.sh));
+}
+
 // narrow rows (<= 128 bytes): several rows per warp (spmm_hop_multirow_kernel), geometry from the small-C sweep of
 // tools/spmm_sweep.cu
-template <typename T, int VEC, int L, int GS, int U, int MINB>
-static int launch_multirow(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst,
-                           int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh) {
-  constexpr int THREADS = 256, HINT = 3;
+template <typename T, int L, int GS, int U, int MINB>
+static int launch_multirow(const HopArgs<T>& h) {
+  constexpr int VEC = 16 / sizeof(T), THREADS = 256, HINT = 3;
   auto kern = spmm_hop_multirow_kernel<T, VEC, L, GS, U, THREADS, MINB, HINT>;
-  if (n_rows == 0) return B200GF_OK;
-  constexpr int rows_per_block = (THREADS / 32) * (32 / GS);
-  int occ = 0;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, 0));
-  if (occ < 1) occ = 1;
-  int64_t blocks = (n_rows + rows_per_block - 1) / rows_per_block;
-  const int64_t cap = (int64_t)sm_count * occ;
-  if (blocks > cap) blocks = cap;
-  kern<<<(unsigned)blocks, THREADS, 0, st>>>(A.rowptr, A.col, reinterpret_cast<const T*>(A.val), src, src_ld, dst,
-                                             dst_ld, n_rows, C, make_scatter<T>(sh));
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  return launch_resident(kern, THREADS, h, h.n_rows, (THREADS / 32) * (32 / GS), 1, h.A.rowptr, h.A.col,
+                         reinterpret_cast<const T*>(h.A.val), h.src, h.src_ld, h.dst, h.dst_ld, h.n_rows, h.C,
+                         make_scatter<T>(h.sh));
 }
 
 // Round-2 kernel (spmm_kernels.cuh: spmm_hop_v2_kernel): 32-byte lanes loaded as two 16-byte halves, 32-bit index
@@ -109,72 +128,30 @@ static int launch_multirow(int sm_count, const CsrDev& A, int64_t n_rows, const 
 // rest (LaneMap; the NVLink epilogues keep a lane's 32 bytes adjacent), so every LDG.128 / STG.128 of a lane group covers
 // whole 32-byte sectors; 32/L neighbours per warp-wide load, U loads in flight per lane; 4 blocks of 256 threads per SM
 // (64 registers); column chunks on blockIdx.y.
-template <typename T, int L, int SCATTER>
-static int launch_v2(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst, int64_t dst_ld,
-                     int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
+template <typename T, int L, int EPI>
+static int launch_v2(const HopArgs<T>& h) {
   constexpr int VEC = 32 / sizeof(T), U = 4, THREADS = 256, MINB = sizeof(T) == 4 ? 4 : 3, HINT = B200GF_HOP_L2_HINT;
   // streaming stores (SH = 1): the result rows are read by the next launch, not by this one, so at normal priority they
   // only displace gathered lines from the L2 (2.74 against 2.78 ms per hop at N = 1M, 64 fp32 columns)
-  auto kern = spmm_hop_v2_kernel<T, int32_t, VEC, L, U, THREADS, MINB, HINT, SCATTER, 1>;
-  if (n_rows == 0) return B200GF_OK;
-  const int n_chunks = (C + L * VEC - 1) / (L * VEC);
+  auto kern = spmm_hop_v2_kernel<T, int32_t, VEC, L, U, THREADS, MINB, HINT, EPI, 1>;
+  const int n_chunks = (h.C + L * VEC - 1) / (L * VEC);
   if (n_chunks > 65535) return B200GF_EUNSUPPORTED;
-  const int wpb = THREADS / 32;
-  int occ = 0;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, 0));
-  if (occ < 1) occ = 1;
-  int64_t blocks = (n_rows + wpb - 1) / wpb;
   // one resident wave per chunk when there is a single chunk; with several chunks each chunk gets its own wave-sized
   // slice of the grid so that the block scheduler runs them chunk-major
-  const int64_t cap = (int64_t)sm_count * occ;
-  if (blocks > cap) blocks = cap;
-  ScatterParam<T, SCATTER> sp{};
-  if constexpr (SCATTER == EPI_SCATTER) sp.a = make_scatter<T>(sh);
-  if constexpr (SCATTER == EPI_BCAST) sp.a = make_bcast<T>(bh);
-  if constexpr (SCATTER == EPI_GRID) { sp.s = make_scatter<T>(sh); sp.a = make_bcast<T>(bh); }
-  kern<<<dim3((unsigned)blocks, (unsigned)n_chunks), THREADS, 0, st>>>(A.rowptr32, A.col, reinterpret_cast<const T*>(A.val),
-                                                                      src, (int)src_ld, dst, (int)dst_ld, (int)n_rows, C,
-                                                                      B200GF_HOP_L2_FRAC, sp);
-  LAUNCH_CHECK();
-  return B200GF_OK;
-}
-
-template <typename T, int L>
-static int launch_v2_sc(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst,
-                        int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
-  if (bh && sh) return launch_v2<T, L, EPI_GRID>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
-  if (bh) return launch_v2<T, L, EPI_BCAST>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, nullptr, bh);
-  if (sh && sh->n_peers > 0) {
-    // the feature-sharded scatter sizes its chunks by row width alone (hop_chunk_lanes without an L2 budget), so L >= 8:
-    // no 4-lane scatter kernel is compiled
-    if constexpr (L >= 8) return launch_v2<T, L, EPI_SCATTER>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
-    else return B200GF_EUNSUPPORTED;
-  }
-  return launch_v2<T, L, EPI_NONE>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, nullptr, nullptr);
+  return launch_resident(kern, THREADS, h, h.n_rows, THREADS / 32, n_chunks, h.A.rowptr32, h.A.col,
+                         reinterpret_cast<const T*>(h.A.val), h.src, (int)h.src_ld, h.dst, (int)h.dst_ld, (int)h.n_rows,
+                         h.C, B200GF_HOP_L2_FRAC, make_epilogue<T, EPI>(h.sh, h.bh));
 }
 
 // 64-byte rows (C = 16 floats / 8 doubles) with 32-byte lanes: two lanes per neighbour row, 8-lane row groups, two loads in
 // flight per lane; rows of C = 8 stay on spmm_hop_multirow_kernel.
-template <typename T, int SCATTER>
-static int launch_multirow_v2(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst,
-                              int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh = nullptr) {
+template <typename T, int EPI>
+static int launch_multirow_v2(const HopArgs<T>& h) {
   constexpr int VEC = 32 / sizeof(T), L = 2, GS = 8, U = 2, THREADS = 256, MINB = sizeof(T) == 4 ? 4 : 3, HINT = 3;
-  auto kern = spmm_hop_multirow_v2_kernel<T, int32_t, VEC, L, GS, U, THREADS, MINB, HINT, SCATTER>;
-  if (n_rows == 0) return B200GF_OK;
-  constexpr int rows_per_block = (THREADS / 32) * (32 / GS);
-  int occ = 0;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, 0));
-  if (occ < 1) occ = 1;
-  int64_t blocks = (n_rows + rows_per_block - 1) / rows_per_block;
-  const int64_t cap = (int64_t)sm_count * occ;
-  if (blocks > cap) blocks = cap;
-  ScatterParam<T, SCATTER> sp{};
-  if constexpr (SCATTER == EPI_SCATTER) sp.a = make_scatter<T>(sh);
-  if constexpr (SCATTER == EPI_GRID) { sp.s = make_scatter<T>(sh); sp.a = make_bcast<T>(bh); }
-  kern<<<(unsigned)blocks, THREADS, 0, st>>>(A.rowptr32, A.col, reinterpret_cast<const T*>(A.val), src, (int)src_ld, dst,
-                                             (int)dst_ld, (int)n_rows, C, sp);
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  auto kern = spmm_hop_multirow_v2_kernel<T, int32_t, VEC, L, GS, U, THREADS, MINB, HINT, EPI>;
+  return launch_resident(kern, THREADS, h, h.n_rows, (THREADS / 32) * (32 / GS), 1, h.A.rowptr32, h.A.col,
+                         reinterpret_cast<const T*>(h.A.val), h.src, (int)h.src_ld, h.dst, (int)h.dst_ld, (int)h.n_rows,
+                         h.C, make_epilogue<T, EPI>(h.sh, h.bh));
 }
 
 // Lane count L (chunk = L x 32 bytes of each row) of spmm_hop_v2_kernel for rows of nw 32-byte vectors.  The kernel runs
@@ -208,33 +185,23 @@ static int hop_chunk_lanes(int64_t n_src, int nw, int64_t l2_bytes, bool spread)
 // own a row's chunk and a warp works on 32 / GS rows (spmm_hop_multirow_v2_kernel); a window holds few entries per row,
 // so that with GS = 4 a row needs no cross-lane fold.  Written columns: [0, padded(C)), as the plain hop.
 template <typename T, int MODE>
-static int launch_window(int sm_count, const int32_t* rowptr, const CsrDev& A, int64_t n_rows, const T* src,
-                         int64_t src_ld, T* dst, int64_t dst_ld, int C, cudaStream_t st) {
+static int launch_window(const HopArgs<T>& h, const int32_t* rowptr, int c0, int Cc) {
   constexpr int VEC = 32 / sizeof(T), L = 4, GS = B200GF_HOP_WIN_GS, U = B200GF_HOP_WIN_U, THREADS = 256;
   constexpr int MINB = sizeof(T) == 4 ? 4 : 3, HINT = B200GF_HOP_WIN_HINT;
   auto kern = spmm_hop_multirow_v2_kernel<T, int32_t, VEC, L, GS, U, THREADS, MINB, HINT, MODE>;
-  constexpr int rows_per_block = (THREADS / 32) * (32 / GS);
-  int occ = 0;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, 0));
-  if (occ < 1) occ = 1;
-  const int64_t blocks = std::min<int64_t>((n_rows + rows_per_block - 1) / rows_per_block, (int64_t)sm_count * occ);
-  kern<<<(unsigned)blocks, THREADS, 0, st>>>(rowptr, A.win_col, reinterpret_cast<const T*>(A.win_val), src, (int)src_ld,
-                                             dst, (int)dst_ld, (int)n_rows, C, ScatterParam<T, MODE>{});
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  return launch_resident(kern, THREADS, h, h.n_rows, (THREADS / 32) * (32 / GS), 1, rowptr, h.A.win_col,
+                         reinterpret_cast<const T*>(h.A.win_val), h.src + c0, (int)h.src_ld, h.dst + c0, (int)h.dst_ld,
+                         (int)h.n_rows, Cc, ScatterParam<T, MODE>{});
 }
 
 template <typename T>
-static int launch_windows(int sm_count, const CsrDev& A, int64_t n_rows, const T* src, int64_t src_ld, T* dst,
-                          int64_t dst_ld, int C, cudaStream_t st) {
-  if (n_rows == 0) return B200GF_OK;
+static int launch_windows(const HopArgs<T>& h) {
   constexpr int CW = 128 / sizeof(T);   // columns per chunk
-  for (int c0 = 0; c0 < C; c0 += CW) {
-    const int Cc = std::min(CW, C - c0);
-    for (int w = 0; w < A.n_win; ++w) {
-      const int32_t* rp = A.win_rowptr32 + (int64_t)w * (n_rows + 1);
-      const int rc = w == 0 ? launch_window<T, EPI_NONE>(sm_count, rp, A, n_rows, src + c0, src_ld, dst + c0, dst_ld, Cc, st)
-                            : launch_window<T, EPI_ACCUM>(sm_count, rp, A, n_rows, src + c0, src_ld, dst + c0, dst_ld, Cc, st);
+  for (int c0 = 0; c0 < h.C; c0 += CW) {
+    const int Cc = std::min(CW, h.C - c0);
+    for (int w = 0; w < h.A.n_win; ++w) {
+      const int32_t* rp = h.A.win_rowptr32 + (int64_t)w * (h.n_rows + 1);
+      const int rc = w == 0 ? launch_window<T, EPI_NONE>(h, rp, c0, Cc) : launch_window<T, EPI_ACCUM>(h, rp, c0, Cc);
       if (rc) return rc;
     }
   }
@@ -257,93 +224,122 @@ int64_t hop_window_rows(int64_t n_src, int64_t l2_bytes, bool spread) {
   return R > 0 && n_src <= 8 * R ? R : 0;
 }
 
+static bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// The operands of 32-byte lanes (the v2 kernels and the windowed hop): 32-bit row offsets and row count; src, and dst
+// when the hop stores one, 32-byte aligned, with strides of whole 32-byte vectors that hold the padded row and fit
+// int32.
 template <typename T>
-static int launch_typed(int sm_count, int64_t l2_bytes, const CsrDev& A, int64_t n_rows, const void* src_, int64_t src_ld,
-                        void* dst_, int64_t dst_ld, int C, cudaStream_t st, const ScatterHost* sh, const BcastHost* bh) {
-  constexpr int VEC = 16 / sizeof(T);
-  const T* src = reinterpret_cast<const T*>(src_);
-  T* dst = reinterpret_cast<T*>(dst_);
-  if (bh) {
-    // fused all-gather epilogue (EPI_BCAST), or all-gather + scatter (EPI_GRID, when `sh` is given too): v2 kernels only
-    // (32-byte aligned rows on every side, 32-bit offsets, rows of at least 64 bytes)
-    constexpr int VWb = 32 / sizeof(T);
-    const int Cwb = (C + VWb - 1) / VWb * VWb;
-    const bool grid = sh && sh->n_peers > 0;
-    bool ok = A.rowptr32 != nullptr && src_ld % VWb == 0 && Cwb <= src_ld && (reinterpret_cast<uintptr_t>(src) & 31) == 0 &&
-              src_ld <= INT32_MAX && n_rows <= INT32_MAX && Cwb >= 2 * VWb;
-    if (bh->n_peers > 0) ok = ok && Cwb <= bh->out_ld && bh->out_ld % VWb == 0;
-    for (int i = 0; i < bh->n_peers; ++i) ok = ok && (reinterpret_cast<uintptr_t>(bh->peer[i]) & 31) == 0;
-    ok = ok && (reinterpret_cast<uintptr_t>(bh->mc) & 31) == 0;
-    if (grid) ok = ok && sh->gl % VWb == 0 && sh->out_ld % VWb == 0 && sh->out_col % VWb == 0 && sh->stride_b % VWb == 0;
-    if (!grid && bh->n_peers <= 0) ok = false;
-    if (dst_) ok = ok && dst_ld % VWb == 0 && Cwb <= dst_ld && (reinterpret_cast<uintptr_t>(dst_) & 31) == 0 && dst_ld <= INT32_MAX;
-    if (!ok) return B200GF_EUNSUPPORTED;
-    const int nwb = Cwb / VWb;
-    if (nwb == 2) {
-      if (!grid) return B200GF_EUNSUPPORTED;        // 64-byte rows: only the grid epilogue is instantiated for the multi-row kernel
-      return launch_multirow_v2<T, EPI_GRID>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
-    }
-    if (nwb <= 4) return launch_v2_sc<T, 4>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, grid ? sh : nullptr, bh);
-    if (nwb <= 8) return launch_v2_sc<T, 8>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, grid ? sh : nullptr, bh);
-    if (nwb <= 16) return launch_v2_sc<T, 16>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, grid ? sh : nullptr, bh);
-    return launch_v2_sc<T, 32>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, grid ? sh : nullptr, bh);
+static bool lanes32_ok(const HopArgs<T>& h) {
+  constexpr int V32 = 32 / sizeof(T);
+  const int64_t Cw = (h.C + V32 - 1) / V32 * V32;
+  const auto rows_ok = [&](const void* p, int64_t ld) {
+    return aligned(p, 32) && ld % V32 == 0 && Cw <= ld && ld <= INT32_MAX;
+  };
+  return h.A.rowptr32 != nullptr && h.n_rows <= INT32_MAX && rows_ok(h.src, h.src_ld) &&
+         (!h.dst || rows_ok(h.dst, h.dst_ld));
+}
+
+// no scatter epilogue, or one whose column offsets and strides are whole vectors of q elements
+static bool scatter_aligned(const ScatterHost* sh, int q) {
+  return !sh || (sh->gl % q == 0 && sh->out_ld % q == 0 && sh->out_col % q == 0 && sh->stride_b % q == 0);
+}
+
+enum class HopKernel { scalar, v1, multirow, multirow_v2, v2, windowed };
+
+struct HopRoute {
+  HopKernel kernel;
+  int L;     // lanes (v1, v2) or 16-byte vectors per row (multirow)
+  int epi;   // EPI_*; the 16-byte-lane kernels take the scatter as ScatterArgs
+};
+
+// The hop's kernel, or B200GF_EUNSUPPORTED, decided before any CUDA call.  The order of the checks is the policy.
+template <typename T>
+static int route_hop(const HopArgs<T>& h, int64_t l2_bytes, HopRoute* r) {
+  constexpr int V16 = 16 / sizeof(T), V32 = 32 / sizeof(T);
+  const int nw = (h.C + V32 - 1) / V32;   // 32-byte vectors per row
+  const bool lanes32 = lanes32_ok(h);
+  if (h.bh) {
+    // 1. fused all-gather (EPI_BCAST), or all-gather + scatter (EPI_GRID): 32-byte lanes into 32-byte aligned peers,
+    //    rows of at least 64 bytes
+    const BcastHost& b = *h.bh;
+    bool ok = lanes32 && nw >= 2 && aligned(b.mc, 32) && scatter_aligned(h.sh, V32);
+    if (b.n_peers > 0) ok = ok && (int64_t)nw * V32 <= b.out_ld && b.out_ld % V32 == 0;
+    for (int i = 0; i < b.n_peers; ++i) ok = ok && aligned(b.peer[i], 32);
+    // 64-byte rows take the multi-row kernel, which is compiled for the grid epilogue only
+    if (!ok || (nw == 2 && !h.sh)) return B200GF_EUNSUPPORTED;
+    *r = nw == 2 ? HopRoute{HopKernel::multirow_v2, 2, EPI_GRID}
+                 : HopRoute{HopKernel::v2, nw <= 4 ? 4 : nw <= 8 ? 8 : nw <= 16 ? 16 : 32, h.sh ? EPI_GRID : EPI_BCAST};
+    return B200GF_OK;
   }
-  const int Cv = (C + VEC - 1) / VEC * VEC;
-  const bool vec_ok = (src_ld % VEC == 0) && (dst_ld % VEC == 0) && (Cv <= src_ld) && (Cv <= dst_ld) &&
-                      ((reinterpret_cast<uintptr_t>(src) & 15) == 0) && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0);
-  if (!vec_ok) {
-    if (sh && sh->n_peers > 0) return B200GF_EUNSUPPORTED;  // the fused scatter needs the 16-byte vector path
-    return launch_one<T, 1, 32, 4>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, nullptr);
+  // 2. 16-byte vectors, else one element per lane (without the fused scatter, which needs the vectors)
+  const int nv = (h.C + V16 - 1) / V16;   // 16-byte vectors per row
+  const auto vec16 = [&](const void* p, int64_t ld) { return aligned(p, 16) && ld % V16 == 0 && nv * V16 <= ld; };
+  if (!vec16(h.src, h.src_ld) || !vec16(h.dst, h.dst_ld)) {
+    if (h.sh) return B200GF_EUNSUPPORTED;
+    *r = {HopKernel::scalar, 32, EPI_NONE};
+    return B200GF_OK;
   }
-  if (sh && sh->n_peers > 0 && (sh->gl % VEC != 0 || sh->out_ld % VEC != 0 || sh->out_col % VEC != 0 || sh->stride_b % VEC != 0))
-    return B200GF_EUNSUPPORTED;
-  const int nv = Cv / VEC;  // 16-byte vectors per row
-  constexpr int MB = sizeof(T) == 4 ? 6 : 4;
-  {
-    // exactly-64-byte rows: the 32-byte-lane multi-row kernel when its preconditions hold
-    constexpr int VW2 = 32 / sizeof(T);
-    bool w2 = nv > 2 && nv <= 4 && A.rowptr32 != nullptr && src_ld % VW2 == 0 && dst_ld % VW2 == 0 && 2 * VW2 <= src_ld &&
-              2 * VW2 <= dst_ld && (reinterpret_cast<uintptr_t>(src) & 31) == 0 && (reinterpret_cast<uintptr_t>(dst) & 31) == 0 &&
-              src_ld <= INT32_MAX && dst_ld <= INT32_MAX && n_rows <= INT32_MAX;
-    if (sh && sh->n_peers > 0)
-      w2 = w2 && sh->gl % VW2 == 0 && sh->out_ld % VW2 == 0 && sh->out_col % VW2 == 0 && sh->stride_b % VW2 == 0;
-    if (w2) {
-      if (sh && sh->n_peers > 0) return launch_multirow_v2<T, EPI_SCATTER>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
-      return launch_multirow_v2<T, EPI_NONE>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, nullptr);
-    }
+  // 3. scatter fields of whole 16-byte vectors
+  if (!scatter_aligned(h.sh, V16)) return B200GF_EUNSUPPORTED;
+  const bool v2_ok = lanes32 && scatter_aligned(h.sh, V32);
+  const int epi = h.sh ? EPI_SCATTER : EPI_NONE;
+  if (nv > 2 && nv <= 4 && v2_ok)
+    *r = {HopKernel::multirow_v2, 2, epi};   // 4. 64-byte rows (C = 16 floats / 8 doubles) with 32-byte lanes
+  else if (nv >= 8 && h.A.n_win > 0 && l2_bytes > 0 && !h.sh && lanes32)
+    *r = {HopKernel::windowed, 4, EPI_NONE};   // 5. rows of at least 128 bytes of an operator with source windows
+  else if (nv <= 8)
+    *r = {HopKernel::multirow, nv <= 1 ? 1 : nv <= 2 ? 2 : nv <= 4 ? 4 : 8, epi};   // 6. rows of <= 128 bytes
+  else if (v2_ok)   // 7. wider rows with 32-byte lanes; the scatter keeps the chunk width of its row width
+    *r = {HopKernel::v2, hop_chunk_lanes(h.n_rows, nw, h.sh ? 0 : l2_bytes, h.A.spread), epi};
+  else
+    *r = {HopKernel::v1, nv <= 16 ? 16 : 32, epi};   // 8. wider rows with 16-byte lanes
+  return B200GF_OK;
+}
+
+// f(std::integral_constant<int, V>{}) for the V of Vs equal to v
+template <int... Vs, typename Fn>
+static int with_const(int v, Fn&& f) {
+  int rc = B200GF_EUNSUPPORTED;
+  (void)((v == Vs && ((rc = f(std::integral_constant<int, Vs>{})), true)) || ...);
+  return rc;
+}
+
+// the instantiation of a route
+template <typename T>
+static int launch_route(const HopArgs<T>& h, const HopRoute& r) {
+  constexpr int V16 = 16 / sizeof(T), MB = sizeof(T) == 4 ? 6 : 4;
+  const auto with_epi = [&](auto f) { return with_const<EPI_NONE, EPI_SCATTER, EPI_BCAST, EPI_GRID>(r.epi, f); };
+  switch (r.kernel) {
+    case HopKernel::scalar: return launch_one<T, 1, 32>(h);
+    case HopKernel::v1: return r.L == 16 ? launch_one<T, V16, 16>(h) : launch_one<T, V16, 32>(h);
+    case HopKernel::multirow:
+      switch (r.L) {
+        case 1: return launch_multirow<T, 1, 8, 1, MB>(h);
+        case 2: return launch_multirow<T, 2, 8, 2, MB>(h);
+        case 4: return launch_multirow<T, 4, 16, 2, sizeof(T) == 4 ? 8 : 4>(h);
+        default: return launch_multirow<T, 8, 32, 4, MB>(h);
+      }
+    case HopKernel::multirow_v2:
+      return with_epi([&](auto e) -> int {
+        constexpr int EPI = decltype(e)::value;
+        // the all-gather alone never takes 64-byte rows: no such multi-row kernel is compiled
+        if constexpr (EPI == EPI_BCAST) return B200GF_EUNSUPPORTED;
+        else return launch_multirow_v2<T, EPI>(h);
+      });
+    case HopKernel::v2:
+      return with_const<4, 8, 16, 32>(r.L, [&](auto l) {
+        return with_epi([&](auto e) -> int {
+          constexpr int L = decltype(l)::value, EPI = decltype(e)::value;
+          // the scatter alone sizes its chunks by row width (hop_chunk_lanes without an L2 budget), so L >= 8: no 4-lane
+          // scatter kernel is compiled
+          if constexpr (L == 4 && EPI == EPI_SCATTER) return B200GF_EUNSUPPORTED;
+          else return launch_v2<T, L, EPI>(h);
+        });
+      });
+    case HopKernel::windowed: return launch_windows<T>(h);
   }
-  // rows of at least 128 bytes of an operator with a window-major copy: the windowed hop (32-byte aligned rows, 32-bit
-  // offsets), unless the plan's L2 size is 0 or the scatter epilogue is fused
-  if (A.n_win > 0 && nv >= 8 && l2_bytes > 0 && !(sh && sh->n_peers > 0)) {
-    constexpr int VW = 32 / sizeof(T);
-    const int Cw = (C + VW - 1) / VW * VW;
-    if (src_ld % VW == 0 && dst_ld % VW == 0 && Cw <= src_ld && Cw <= dst_ld && (reinterpret_cast<uintptr_t>(src) & 31) == 0 &&
-        (reinterpret_cast<uintptr_t>(dst) & 31) == 0 && src_ld <= INT32_MAX && dst_ld <= INT32_MAX && n_rows <= INT32_MAX)
-      return launch_windows<T>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st);
-  }
-  if (nv <= 1) return launch_multirow<T, VEC, 1, 8, 1, MB>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
-  if (nv <= 2) return launch_multirow<T, VEC, 2, 8, 2, MB>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
-  if (nv <= 4) return launch_multirow<T, VEC, 4, 16, 2, sizeof(T) == 4 ? 8 : 4>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
-  if (nv <= 8) return launch_multirow<T, VEC, 8, 32, 4, MB>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
-  // rows wider than 128 bytes: the v2 kernel when its preconditions hold (32-byte aligned rows, 32-bit offsets)
-  constexpr int VW = 32 / sizeof(T);
-  const int Cw = (C + VW - 1) / VW * VW;
-  bool wide_ok = A.rowptr32 != nullptr && (src_ld % VW == 0) && (dst_ld % VW == 0) && (Cw <= src_ld) && (Cw <= dst_ld) &&
-                 ((reinterpret_cast<uintptr_t>(src) & 31) == 0) && ((reinterpret_cast<uintptr_t>(dst) & 31) == 0) &&
-                 src_ld <= INT32_MAX && dst_ld <= INT32_MAX && n_rows <= INT32_MAX;
-  if (sh && sh->n_peers > 0)
-    wide_ok = wide_ok && sh->gl % VW == 0 && sh->out_ld % VW == 0 && sh->out_col % VW == 0 && sh->stride_b % VW == 0;
-  if (wide_ok) {
-    const int nw = Cw / VW;  // 32-byte vectors per row
-    // the feature-sharded scatter keeps the chunk width of its row width
-    const int L = hop_chunk_lanes(n_rows, nw, sh && sh->n_peers > 0 ? 0 : l2_bytes, A.spread);
-    if (L == 4) return launch_v2_sc<T, 4>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
-    if (L == 8) return launch_v2_sc<T, 8>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
-    if (L == 16) return launch_v2_sc<T, 16>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
-    return launch_v2_sc<T, 32>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, nullptr);
-  }
-  if (nv <= 16) return launch_one<T, VEC, 16, 4>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
-  return launch_one<T, VEC, 32, 4>(sm_count, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh);
+  return B200GF_EUNSUPPORTED;
 }
 
 int launch_hop(int dtype, int sm_count, int64_t l2_bytes, const CsrDev& A, int64_t n_rows, const void* src,
@@ -352,8 +348,13 @@ int launch_hop(int dtype, int sm_count, int64_t l2_bytes, const CsrDev& A, int64
   if (sh && (sh->n_peers < 0 || sh->n_peers > MAX_PEERS)) return B200GF_EINVAL;
   if (bh && (bh->n_peers < 0 || bh->n_peers > MAX_PEERS || (bh->n_peers > 0 && bh->out_ld < C))) return B200GF_EINVAL;
   if (bh && bh->n_peers == 0 && !(sh && sh->n_peers > 0)) return B200GF_EINVAL;   // no all-gather only in the grid epilogue
-  return with_dtype(dtype, [&](auto tag) {
-    return launch_typed<decltype(tag)>(sm_count, l2_bytes, A, n_rows, src, src_ld, dst, dst_ld, C, st, sh, bh);
+  return with_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    const HopArgs<T> h{sm_count, A, n_rows, reinterpret_cast<const T*>(src), src_ld, reinterpret_cast<T*>(dst), dst_ld, C, st,
+                       sh && sh->n_peers > 0 ? sh : nullptr, bh};
+    HopRoute r;
+    if (int rc = route_hop(h, l2_bytes, &r)) return rc;
+    return n_rows == 0 ? B200GF_OK : launch_route(h, r);
   });
 }
 
@@ -378,17 +379,14 @@ int launch_bcast_rows(int dtype, const void* src, int64_t src_ld, int64_t n_rows
   if ((reinterpret_cast<uintptr_t>(src) & 15) || (reinterpret_cast<uintptr_t>(bh->mc) & 15)) return B200GF_EUNSUPPORTED;
   for (int i = 0; i < bh->n_peers; ++i)   // 16-byte vector stores into every peer
     if (reinterpret_cast<uintptr_t>(bh->peer[i]) & 15) return B200GF_EUNSUPPORTED;
-  if (dtype == B200GF_F32) {
-    if (C % 4 || src_ld % 4 || bh->out_ld % 4) return B200GF_EUNSUPPORTED;
-    bcast_rows_kernel<float, 4><<<blocks, 256, 0, st>>>((const float*)src, src_ld, n_rows, C, make_bcast<float>(bh));
-  } else if (dtype == B200GF_F64) {
-    if (C % 2 || src_ld % 2 || bh->out_ld % 2) return B200GF_EUNSUPPORTED;
-    bcast_rows_kernel<double, 2><<<blocks, 256, 0, st>>>((const double*)src, src_ld, n_rows, C, make_bcast<double>(bh));
-  } else {
-    return B200GF_EUNSUPPORTED;
-  }
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  return with_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    constexpr int VEC = 16 / sizeof(T);
+    if (C % VEC || src_ld % VEC || bh->out_ld % VEC) return B200GF_EUNSUPPORTED;
+    bcast_rows_kernel<T, VEC><<<blocks, 256, 0, st>>>((const T*)src, src_ld, n_rows, C, make_bcast<T>(bh));
+    LAUNCH_CHECK();
+    return B200GF_OK;
+  });
 }
 
 // copy-scatter of an existing node-major matrix (the k = 0 term, x itself) into the peers' row-local operands
@@ -411,28 +409,32 @@ int launch_scatter_rows(int dtype, const void* src, int64_t src_ld, int64_t n_ro
   if (n_rows == 0) return B200GF_OK;
   const int blocks = 132 * 8;
   if (reinterpret_cast<uintptr_t>(src) & 15) return B200GF_EUNSUPPORTED;   // 16-byte vector loads
-  if (dtype == B200GF_F32) {
-    if (C % 4 || src_ld % 4 || sh->gl % 4 || sh->out_ld % 4 || sh->out_col % 4 || sh->stride_b % 4) return B200GF_EUNSUPPORTED;
-    scatter_rows_kernel<float, 4><<<blocks, 256, 0, st>>>((const float*)src, src_ld, n_rows, C, make_scatter<float>(sh));
-  } else if (dtype == B200GF_F64) {
-    if (C % 2 || src_ld % 2 || sh->gl % 2 || sh->out_ld % 2 || sh->out_col % 2 || sh->stride_b % 2) return B200GF_EUNSUPPORTED;
-    scatter_rows_kernel<double, 2><<<blocks, 256, 0, st>>>((const double*)src, src_ld, n_rows, C, make_scatter<double>(sh));
-  } else {
-    return B200GF_EUNSUPPORTED;
-  }
-  LAUNCH_CHECK();
-  return B200GF_OK;
+  return with_dtype(dtype, [&](auto tag) -> int {
+    using T = decltype(tag);
+    constexpr int VEC = 16 / sizeof(T);
+    if (C % VEC || src_ld % VEC || !scatter_aligned(sh, VEC)) return B200GF_EUNSUPPORTED;
+    scatter_rows_kernel<T, VEC><<<blocks, 256, 0, st>>>((const T*)src, src_ld, n_rows, C, make_scatter<T>(sh));
+    LAUNCH_CHECK();
+    return B200GF_OK;
+  });
 }
 
 }  // namespace b200gf
 
+// the operator of (e, direction) of a plan, null for a null plan, an e out of range, an unknown direction, or the
+// backward operator of a plan without one
+static const b200gf::CsrDev* hop_operator(const b200gf_plan* plan, int e, int direction) {
+  if (!plan || e < 0 || e >= plan->E) return nullptr;
+  if (direction == B200GF_HOP_FWD) return &plan->fwd[e];
+  if (direction == B200GF_HOP_BWD && plan->has_bwd) return &plan->bwd[e];
+  return nullptr;
+}
+
 extern "C" int b200gf_hop(const b200gf_plan* plan, int e, int direction, const void* src, int64_t src_ld,
                           void* dst, int64_t dst_ld, int C, void* stream) {
-  if (!plan || !src || !dst || e < 0 || e >= plan->E) return B200GF_EINVAL;
-  if (direction != B200GF_HOP_FWD && direction != B200GF_HOP_BWD) return B200GF_EINVAL;
-  if (direction == B200GF_HOP_BWD && !plan->has_bwd) return B200GF_EINVAL;
-  const b200gf::CsrDev& A = direction == B200GF_HOP_FWD ? plan->fwd[e] : plan->bwd[e];
-  return b200gf::plan_hop(plan, A, src, src_ld, dst, dst_ld, C, (cudaStream_t)stream, nullptr);
+  const b200gf::CsrDev* A = hop_operator(plan, e, direction);
+  if (!A || !src || !dst) return B200GF_EINVAL;
+  return b200gf::plan_hop(plan, *A, src, src_ld, dst, dst_ld, C, (cudaStream_t)stream, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -454,15 +456,13 @@ extern "C" int b200gf_hop_scatter(const b200gf_plan* plan, int e, int direction,
                                   void* dst, int64_t dst_ld, int C, const void* const* peers, int n_peers,
                                   int64_t rows_per_peer, int64_t out_ld, int64_t out_col, int gl, int64_t stride_b,
                                   void* stream) {
-  if (!plan || !src || !dst || e < 0 || e >= plan->E) return B200GF_EINVAL;
-  if (direction != B200GF_HOP_FWD && direction != B200GF_HOP_BWD) return B200GF_EINVAL;
-  if (direction == B200GF_HOP_BWD && !plan->has_bwd) return B200GF_EINVAL;
+  const b200gf::CsrDev* A = hop_operator(plan, e, direction);
+  if (!A || !src || !dst) return B200GF_EINVAL;
   b200gf::ScatterHost sh{};
   int rc = fill_scatter(sh, peers, n_peers, rows_per_peer, out_ld, out_col, gl, stride_b);
   if (rc) return rc;
   if (plan->n_rows > rows_per_peer * n_peers || C % gl != 0) return B200GF_EINVAL;
-  const b200gf::CsrDev& A = direction == B200GF_HOP_FWD ? plan->fwd[e] : plan->bwd[e];
-  return b200gf::plan_hop(plan, A, src, src_ld, dst, dst_ld, C, (cudaStream_t)stream, &sh);
+  return b200gf::plan_hop(plan, *A, src, src_ld, dst, dst_ld, C, (cudaStream_t)stream, &sh);
 }
 
 extern "C" int b200gf_scatter_rows(int dtype, const void* src, int64_t src_ld, int64_t n_rows, int C,
@@ -489,23 +489,20 @@ static int fill_bcast(b200gf::BcastHost& bh, const void* const* peers, int n_pee
 extern "C" int b200gf_hop_bcast(const b200gf_plan* plan, int e, int direction, const void* src, int64_t src_ld, int C,
                                 const void* const* peers, int n_peers, const void* mc, int64_t row0, int64_t out_ld,
                                 void* stream) {
-  if (!plan || !src || e < 0 || e >= plan->E) return B200GF_EINVAL;
-  if (direction != B200GF_HOP_FWD && direction != B200GF_HOP_BWD) return B200GF_EINVAL;
-  if (direction == B200GF_HOP_BWD && !plan->has_bwd) return B200GF_EINVAL;
+  const b200gf::CsrDev* A = hop_operator(plan, e, direction);
+  if (!A || !src) return B200GF_EINVAL;
   b200gf::BcastHost bh{};
   int rc = fill_bcast(bh, peers, n_peers, mc, row0, out_ld);
   if (rc) return rc;
-  const b200gf::CsrDev& A = direction == B200GF_HOP_FWD ? plan->fwd[e] : plan->bwd[e];
-  return b200gf::plan_hop(plan, A, src, src_ld, nullptr, 0, C, (cudaStream_t)stream, nullptr, &bh);
+  return b200gf::plan_hop(plan, *A, src, src_ld, nullptr, 0, C, (cudaStream_t)stream, nullptr, &bh);
 }
 
 extern "C" int b200gf_hop_grid(const b200gf_plan* plan, int e, int direction, const void* src, int64_t src_ld, int C,
                                const void* const* bc_peers, int n_bc, int64_t row0, int64_t bc_ld,
                                const void* const* sc_peers, int n_sc, int64_t rows_per_peer, int64_t out_ld, int64_t out_col,
                                int gl, int64_t stride_b, void* stream) {
-  if (!plan || !src || e < 0 || e >= plan->E) return B200GF_EINVAL;
-  if (direction != B200GF_HOP_FWD && direction != B200GF_HOP_BWD) return B200GF_EINVAL;
-  if (direction == B200GF_HOP_BWD && !plan->has_bwd) return B200GF_EINVAL;
+  const b200gf::CsrDev* A = hop_operator(plan, e, direction);
+  if (!A || !src) return B200GF_EINVAL;
   b200gf::BcastHost bh{};
   if (n_bc > 0) {
     int rc = fill_bcast(bh, bc_peers, n_bc, nullptr, row0, bc_ld);
@@ -517,8 +514,7 @@ extern "C" int b200gf_hop_grid(const b200gf_plan* plan, int e, int direction, co
   int rc = fill_scatter(sh, sc_peers, n_sc, rows_per_peer, out_ld, out_col, gl, stride_b);
   if (rc) return rc;
   if (plan->n_rows > rows_per_peer * n_sc || C % gl != 0) return B200GF_EINVAL;
-  const b200gf::CsrDev& A = direction == B200GF_HOP_FWD ? plan->fwd[e] : plan->bwd[e];
-  return b200gf::plan_hop(plan, A, src, src_ld, nullptr, 0, C, (cudaStream_t)stream, &sh, &bh);
+  return b200gf::plan_hop(plan, *A, src, src_ld, nullptr, 0, C, (cudaStream_t)stream, &sh, &bh);
 }
 
 extern "C" int b200gf_bcast_rows(int dtype, const void* src, int64_t src_ld, int64_t n_rows, int C,
