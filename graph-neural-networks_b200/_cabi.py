@@ -42,6 +42,9 @@ _SIGNATURES = {
     "b200gf_relu_backward": (c_int, [c_int, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i64, c_int, c_vp]),
     "b200gf_maxpool_forward": (c_int, [c_int, c_vp, c_i64, c_i64, c_int, c_vp, c_i64, c_int, c_vp, c_i64, c_vp, c_vp]),
     "b200gf_maxpool_backward": (c_int, [c_int, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_i64, c_i64, c_vp]),
+    "b200gf_local_activation_forward": (c_int, [c_int, c_int, c_vp, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_int, c_vp,
+                                                c_vp, c_i64, c_vp, c_i64, c_vp, c_vp]),
+    "b200gf_local_activation_backward": (c_int, [c_int, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_i64, c_vp]),
     "b200gf_backward": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_vp, c_int, c_i64, c_vp, c_vp,
                                 c_int, c_vp, c_sz, c_int, c_int, c_int, c_int, c_vp]),
     "b200gf_workspace_bytes": (c_sz, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int]),

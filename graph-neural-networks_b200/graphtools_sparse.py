@@ -12,6 +12,7 @@ scale to the graphs of BASELINE.json's configs.  Host-side numpy/scipy only: thi
     spectral_normalize          S = W / max(real eig), examples/sourceLocGNN.py:752 (via computeGFT :270-309)
     is_connected                graphTools.py:562-589   (components of the symmetrised pattern instead of Laplacian eig)
     compute_neighborhood        graphTools.py:378-527
+    ring_neighborhoods          the K-hop neighbourhoods of compute_neighborhood as one CSR, ordered by hop distance
     perm_degree                 graphTools.py:1020-1052
     edge_fail_sampling          graphTools.py:1163-1190
     sparsify_graph              graphTools.py:591-680
@@ -86,19 +87,24 @@ def is_connected(W):
     return n == 1
 
 
-def compute_neighborhood(S, K, N="all", nb="all", outputType="list"):
-    """K-hop neighbourhoods (graphTools.py:378-527).  S: sparse matrix, or a list of E sparse matrices (edge features:
-    an edge exists where sum_e |S_e| > 0, :424-432).  Row i's one-hop neighbours are the columns j with S[i, j] > 0.
-    Returns, for the first N nodes, the nodes < nb reachable within K hops (each node is in its own neighbourhood):
-    a list of sorted lists, or (outputType 'matrix') an int array padded with the node's own index (:504-525)."""
+def _edge_pattern(S):
+    """Boolean CSR pattern of S, or of a list of E matrices (edge features: an edge exists where sum_e |S_e| > 1e-9,
+    graphTools.py:424-432)."""
     if isinstance(S, (list, tuple)):
         acc = None
         for Se in S:
             Se = abs(_csr(Se))
             acc = Se if acc is None else acc + Se
-        A = (acc > zeroTolerance)
-    else:
-        A = (_csr(S) > zeroTolerance)
+        return acc > zeroTolerance
+    return _csr(S) > zeroTolerance
+
+
+def compute_neighborhood(S, K, N="all", nb="all", outputType="list"):
+    """K-hop neighbourhoods (graphTools.py:378-527).  S: sparse matrix, or a list of E sparse matrices (edge features:
+    an edge exists where sum_e |S_e| > 0, :424-432).  Row i's one-hop neighbours are the columns j with S[i, j] > 0.
+    Returns, for the first N nodes, the nodes < nb reachable within K hops (each node is in its own neighbourhood):
+    a list of sorted lists, or (outputType 'matrix') an int array padded with the node's own index (:504-525)."""
+    A = _edge_pattern(S)
     n = A.shape[0]
     assert K >= 0
     if N == "all":
@@ -125,6 +131,42 @@ def compute_neighborhood(S, K, N="all", nb="all", outputType="list"):
             out[i, len(x):] = i
         return out
     return neighbors
+
+
+def ring_neighborhoods(S, K):
+    """Every node's K-hop neighbourhood (compute_neighborhood's edge rule: row i's neighbours are the columns j with
+    sum_e |S_e[i, j]| > 1e-9) as one CSR ordered by hop distance.  S: sparse matrix or list of E of them.
+
+    Returns (rowptr int64 [N+1], col int32, ring_end int32 [N, K+1]): row i lists col[rowptr[i] : rowptr[i+1]], ring 0
+    (i itself), then ring 1 (the nodes first reached in one hop), ..., ring K, ascending node index within a ring; its
+    k-hop neighbourhood is the prefix of length ring_end[i, k].  This is the list format of the localized activations'
+    kernels (b200gf_local_activation_forward): one list per node serves every k, and no row is padded to the widest."""
+    A = _edge_pattern(S)
+    n = A.shape[0]
+    assert K >= 0
+    step = (A.astype(np.int32) + sp.identity(n, dtype=np.int32, format="csr")).tocsr()
+    reach = sp.identity(n, dtype=np.int32, format="csr")
+    rings = [reach]
+    for _ in range(K):
+        nxt = (reach @ step).tocsr()
+        nxt.data[:] = 1                          # boolean semiring; int32 path counts cannot wrap to zero
+        ring = (nxt - reach).tocsr()             # reach is a subset of nxt (step holds the identity)
+        ring.eliminate_zeros()
+        rings.append(ring)
+        reach = nxt
+    total = int(reach.nnz)
+    if total > np.iinfo(np.int32).max:
+        raise ValueError("ring_neighborhoods: the %d-hop lists of N = %d nodes hold %d entries, more than the 2^31 - 1 "
+                         "that int32 list offsets address" % (K, n, total))
+    counts = np.stack([np.diff(r.indptr) for r in rings], axis=1).astype(np.int64)       # [N, K+1]
+    ring_end = np.cumsum(counts, axis=1)
+    rowptr = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(ring_end[:, -1], out=rowptr[1:])
+    rows = np.concatenate([np.repeat(np.arange(n), np.diff(r.indptr)) for r in rings])
+    hops = np.concatenate([np.full(r.nnz, k, dtype=np.int32) for k, r in enumerate(rings)])
+    cols = np.concatenate([r.indices for r in rings])
+    order = np.lexsort((cols, hops, rows))
+    return rowptr, cols[order].astype(np.int32), ring_end.astype(np.int32)
 
 
 def perm_degree(S):

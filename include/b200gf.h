@@ -160,6 +160,25 @@ int b200gf_maxpool_forward(int dtype, const void* x, int64_t x_ld, int64_t n_in,
 int b200gf_maxpool_backward(int dtype, const void* dy, int64_t dy_ld, const int32_t* argmax, int64_t n_out, int C,
                             void* dx, int64_t dx_ld, int64_t n_in, void* stream);
 
+/* MaxLocalActivation / MedianLocalActivation (alegnn/utils/graphML.py:1535-1810) on node-major data [N, ld]:
+ *   y[i, c] = w[0] x[i, c] + sum_{k=1..K} w[k] agg_k[i, c]      (k ascending; weight: K+1 values in device memory)
+ * agg_k[i, c] is the maximum (select B200GF_LOCAL_MAX) or the lower median, the (n - 1) / 2-th smallest of n
+ * (B200GF_LOCAL_MEDIAN), of x[j, c] over the k-hop neighbourhood of i.  The neighbourhoods are ring-ordered lists:
+ * row i is col[rowptr[i] ..] (rowptr int64 [N+1], col int32), node i first, then its 1-hop ring, ..., its K-hop ring,
+ * ascending node index within a ring; its k-hop neighbourhood is the prefix of length ring_end[i * (K+1) + k] (int32
+ * [N, K+1]).  Ties: the maximum goes to the smallest node index holding it, the median likewise.  NaN inputs give an
+ * unspecified result.  agg receives agg_k at agg + (k-1) N agg_ld, arg (int32 [K, N, C]) the chosen node of every
+ * agg_k element.
+ * The backward sets dx = w[0] dy and adds w[k] dy[i, c] to dx[arg_k[i, c], c] for every k, with atomics: its last
+ * bits may change from run to run.  The weight gradient is left to the caller (sum of x dy and agg_k dy). */
+enum { B200GF_LOCAL_MAX = 0, B200GF_LOCAL_MEDIAN = 1 };
+int b200gf_local_activation_forward(int dtype, int select, const void* x, int64_t x_ld, int64_t N, int C,
+                                    const int64_t* rowptr, const int32_t* col, const int32_t* ring_end, int K,
+                                    const void* weight, void* y, int64_t y_ld, void* agg, int64_t agg_ld, int32_t* arg,
+                                    void* stream);
+int b200gf_local_activation_backward(int dtype, const void* dy, int64_t dy_ld, const int32_t* arg, int64_t N, int C, int K,
+                                     const void* weight, void* dx, int64_t dx_ld, void* stream);
+
 /* LSIGF backward (autograd of the above; SURVEY.md §8 a-8)
  *   V_{e,0} = dy,  V_{e,k} = V_{e,k-1} S_e^T              (K-1 hops with the backward operator)
  *   dx      = sum_{e,k,f} h[f,e,k,g] V_{e,k}[.,f,.]        (NULL to skip)
