@@ -17,6 +17,7 @@ from .arma import jARMA, GraphFilterARMA, ArmaOperator  # noqa: F401,E402
 from .attention import (graphAttention, graphAttentionLSIGF, graphAttentionEVGF, GraphAttentional,  # noqa: F401,E402
                         GraphFilterAttentional, EdgeVariantAttentional)
 from .delayed import LSIGF_DB, GraphFilter_DB, GRNN_DB, HiddenState_DB  # noqa: F401,E402
+from .aggregation import AggregationGNN, MultiNodeAggregationGNN, AggregationOperator  # noqa: F401,E402
 from .graphed import graphed, GraphedForward  # noqa: F401,E402
 
 __all__ = ["EVGF", "EdgeVariantGF", "MaxPoolLocal", "LSIGF", "GraphFilter", "SparseGSO", "Plan", "plan_for", "install", "uninstall", "fuse_layers"]

@@ -360,7 +360,7 @@ def fuse_layers(model):
 _SAVED = {}
 
 
-def install(gml=None, edge_gating=False, node_variant=False, arma=False, attention=False):
+def install(gml=None, edge_gating=False, node_variant=False, arma=False, attention=False, aggregation=False, archit=None):
     """Point `alegnn.utils.graphML.LSIGF`, `.GraphFilter`, `.EVGF`, `.EdgeVariantGF`, the local pooling / activation
     layers and the static-GSO recurrent layers at this package.  `edge_gating=True` also points
     `.EdgeGatedHiddenState` at the sparse edge-gated layer (edgegated.py); by default it stays the reference's.
@@ -371,6 +371,9 @@ def install(gml=None, edge_gating=False, node_variant=False, arma=False, attenti
     functionals `.graphAttention`, `.graphAttentionLSIGF`, `.graphAttentionEVGF` at the sparse attention layers
     (attention.py); by default they stay the reference's.  `.learnAttentionGSO`, which returns a dense tensor, is always
     the reference's.
+    `aggregation=True` also points `alegnn.modules.architectures.AggregationGNN` and `.MultiNodeAggregationGNN` (or those
+    of `archit`, when given) at the sparse aggregation GNNs (aggregation.py).  Both are retargeted: the reference's
+    MultiNodeAggregationGNN looks AggregationGNN up as a module global and would still build a dense GSO copy per node.
 
     `GraphFilter.forward` in the reference looks `LSIGF` up as a module global at call time (graphML.py:2137), so
     this also accelerates its hybrid EdgeVariantGF (:2686), jARMA (:592) and GatedGRNN (:1403,:1461) call sites.
@@ -402,6 +405,13 @@ def install(gml=None, edge_gating=False, node_variant=False, arma=False, attenti
         # sparse Jacobi chains on the S~ plan instead of [F,E,P,G,N,N] dense operators (arma.py)
         gml.jARMA = arma_mod.jARMA
         gml.GraphFilterARMA = arma_mod.GraphFilterARMA
+    if aggregation:
+        from . import aggregation as aggregation_mod
+        if archit is None:
+            import alegnn.modules.architectures as archit
+        for name in ("AggregationGNN", "MultiNodeAggregationGNN"):
+            _SAVED[id(gml)][1].setdefault((archit, name), getattr(archit, name))
+            setattr(archit, name, getattr(aggregation_mod, name))
     if attention:
         names = ("graphAttention", "graphAttentionLSIGF", "graphAttentionEVGF", "GraphAttentional",
                  "GraphFilterAttentional", "EdgeVariantAttentional")
@@ -435,5 +445,6 @@ def uninstall(gml=None):
     for key, (mod, saved) in list(_SAVED.items()):
         if gml is None or mod is gml:
             for name, obj in saved.items():
-                setattr(mod, name, obj)
+                target, attr = name if isinstance(name, tuple) else (mod, name)   # (module, name): another module
+                setattr(target, attr, obj)
             del _SAVED[key]
